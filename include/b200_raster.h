@@ -240,6 +240,46 @@ int b200r_interp_face_attrs_backward(const int64_t* pix_to_face, const float* ba
                                      const float* face_attrs, const float* grad_pix_attrs, int64_t P, int64_t F,
                                      int64_t D, float* grad_barycentric_coords, float* grad_face_attrs, void* stream);
 
+/* ------------------------------------------------------------------ mesh blending ------------------------ */
+
+/*
+ * Replace pytorch3d._C.sigmoid_alpha_blend / sigmoid_alpha_blend_backward
+ *   (SigmoidAlphaBlend / SigmoidAlphaBlendBackward, pytorch3d/csrc/blending/sigmoid_alpha_blend.h;
+ *    call site pytorch3d/renderer/blending.py _SigmoidAlphaBlend).  Bit-identical to the reference's CUDA kernels.
+ *  dists float32 (N,H,W,K); pix_to_face int64 (N,H,W,K) (a slot is empty when the index, read as a 32-bit int, is < 0);
+ *  alphas float32 (N,H,W), fully written: 1 - prod over valid slots of (1 - sigmoid(-dist / sigma)).
+ *  Backward: grad_alphas and alphas (the forward's output) float32 (N,H,W); grad_dists float32 (N,H,W,K), fully
+ *  written (0 in empty slots).
+ */
+int b200r_sigmoid_alpha_blend_forward(const float* dists, const int64_t* pix_to_face, int32_t N, int32_t H, int32_t W,
+                                      int32_t K, float sigma, float* alphas, void* stream);
+int b200r_sigmoid_alpha_blend_backward(const float* grad_alphas, const float* alphas, const float* dists,
+                                       const int64_t* pix_to_face, int32_t N, int32_t H, int32_t W, int32_t K,
+                                       float sigma, float* grad_dists, void* stream);
+
+/*
+ * Fused softmax_rgb_blend (additional entry points, no counterpart in pytorch3d._C): the torch chain of
+ * pytorch3d/renderer/blending.py softmax_rgb_blend in one kernel per direction, on the rasterizer's layout.
+ *  colors float32 (N,H,W,K,3); pix_to_face int64 (N,H,W,K) (valid where >= 0); zbuf, dists float32 (N,H,W,K);
+ *  K <= 150.  sigma, gamma as in BlendParams.
+ *  background: device float32 (3,), or NULL and then background_value: HOST float[3].
+ *  znear / zfar: device float32 (N,) per image, or NULL and then the scalar znear_value / zfar_value (a double, as a
+ *  Python float: the range zfar - znear is formed in double precision, like the Python expression).
+ *  out float32 (N,H,W,4) RGBA, fully written.
+ * Backward: grad_out float32 (N,H,W,4); grad_colors (N,H,W,K,3), grad_dists and grad_zbuf (N,H,W,K) float32, fully
+ * written.  The gradient through the per-pixel maximum of the inverse depth goes to the first slot attaining it.
+ */
+int b200r_softmax_rgb_blend_forward(const float* colors, const int64_t* pix_to_face, const float* zbuf,
+                                    const float* dists, int32_t N, int32_t H, int32_t W, int32_t K, float sigma,
+                                    float gamma, const float* background, const float* background_value,
+                                    const float* znear, const float* zfar, double znear_value, double zfar_value,
+                                    float* out, void* stream);
+int b200r_softmax_rgb_blend_backward(const float* grad_out, const float* colors, const int64_t* pix_to_face,
+                                     const float* zbuf, const float* dists, int32_t N, int32_t H, int32_t W, int32_t K,
+                                     float sigma, float gamma, const float* background, const float* background_value,
+                                     const float* znear, const float* zfar, double znear_value, double zfar_value,
+                                     float* grad_colors, float* grad_dists, float* grad_zbuf, void* stream);
+
 /* ------------------------------------------------------------------ frame exchange between GPUs ---------- */
 
 /*

@@ -594,6 +594,145 @@ def interp_face_attrs_backward(pix_to_face: torch.Tensor, barycentric_coords: to
     return grad_bary, grad_attrs
 
 
+def _check_blend_inputs(named_floats, pix_to_face):
+    dev = _require_cuda(*named_floats, ("pix_to_face", pix_to_face))
+    for name, t in named_floats:
+        if t.dtype != torch.float32:
+            raise RuntimeError("Expected tensor for %s to have scalar type Float; but got %s" % (name, t.dtype))
+    if pix_to_face.dtype != torch.int64:
+        raise RuntimeError("expected scalar type Long but found %s" % pix_to_face.dtype)
+    if pix_to_face.dim() != 4:
+        raise RuntimeError("pix_to_face must have dimensions (N, H, W, K)")
+    return dev
+
+
+def sigmoid_alpha_blend(dists: torch.Tensor, pix_to_face: torch.Tensor, sigma: float):
+    """pytorch3d._C.sigmoid_alpha_blend (SigmoidAlphaBlend, csrc/blending/sigmoid_alpha_blend.h): dists (N,H,W,K) f32,
+    pix_to_face (N,H,W,K) i64 -> alphas (N,H,W) f32, bit-identical to the reference's CUDA kernel."""
+    dev = _check_blend_inputs([("distances", dists)], pix_to_face)
+    if dists.shape != pix_to_face.shape:
+        raise RuntimeError("distances and pix_to_face must both be (N, H, W, K)")
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    dd, p2f = dists.contiguous(), pix_to_face.contiguous()
+    with torch.cuda.device(dev):
+        alphas = torch.empty((N, H, W), dtype=torch.float32, device=dev)
+        if alphas.numel() == 0:
+            return alphas
+        _lib.check(lib.b200r_sigmoid_alpha_blend_forward(_ptr(dd), _ptr(p2f), N, H, W, K, float(sigma), _ptr(alphas),
+                                                         _stream_ptr(dev)))
+    return alphas
+
+
+def sigmoid_alpha_blend_backward(grad_alphas: torch.Tensor, alphas: torch.Tensor, dists: torch.Tensor,
+                                 pix_to_face: torch.Tensor, sigma: float):
+    """pytorch3d._C.sigmoid_alpha_blend_backward (SigmoidAlphaBlendBackward) -> grad_dists (N,H,W,K) f32."""
+    dev = _check_blend_inputs([("grad_alphas", grad_alphas), ("alphas", alphas), ("distances", dists)], pix_to_face)
+    if dists.shape != pix_to_face.shape or alphas.shape != pix_to_face.shape[:3] or grad_alphas.shape != alphas.shape:
+        raise RuntimeError("distances and pix_to_face must be (N, H, W, K); alphas and grad_alphas (N, H, W)")
+    if alphas.numel() == 0:
+        return grad_alphas  # what the reference returns for an empty image (sigmoid_alpha_blend.cu)
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    ga, al, dd, p2f = grad_alphas.contiguous(), alphas.contiguous(), dists.contiguous(), pix_to_face.contiguous()
+    with torch.cuda.device(dev):
+        grad_dists = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
+        if grad_dists.numel() == 0:
+            return grad_dists
+        _lib.check(lib.b200r_sigmoid_alpha_blend_backward(_ptr(ga), _ptr(al), _ptr(dd), _ptr(p2f), N, H, W, K,
+                                                          float(sigma), _ptr(grad_dists), _stream_ptr(dev)))
+    return grad_dists
+
+
+def _softmax_side_args(dev, N, background_color, znear, zfar):
+    """(background ptr, host background value, znear ptr, zfar ptr, znear value, zfar value, tensors to keep alive).
+    Tensors are read on the device; Python numbers go to the kernel as numbers."""
+    import ctypes
+    keep = []
+    if torch.is_tensor(background_color):
+        bg = background_color
+        if bg.device != dev or bg.dtype != torch.float32 or bg.numel() != 3:
+            raise RuntimeError("background_color must be a float32 tensor of 3 values on %s" % dev)
+        bg = bg.reshape(3).contiguous()
+        keep.append(bg)
+        bg_ptr, bg_val = bg.data_ptr(), None
+    else:
+        vals = [float(v) for v in background_color]
+        if len(vals) != 3:
+            raise RuntimeError("background_color must have 3 values")
+        bg_ptr, bg_val = None, (ctypes.c_float * 3)(*vals)
+    ptrs, values = [], []
+    for name, z in (("znear", znear), ("zfar", zfar)):
+        if torch.is_tensor(z):
+            if z.device != dev or z.dtype != torch.float32 or z.dim() != 1 or z.shape[0] not in (1, N):
+                raise RuntimeError("%s must be a number or a float32 tensor of shape (N,) on %s" % (name, dev))
+            z = z.expand(N).contiguous()
+            keep.append(z)
+            ptrs.append(z.data_ptr())
+            values.append(0.0)
+        else:
+            ptrs.append(None)
+            values.append(float(z))
+    return bg_ptr, bg_val, ptrs[0], ptrs[1], values[0], values[1], keep
+
+
+def _check_softmax_inputs(colors, pix_to_face, zbuf, dists):
+    dev = _check_blend_inputs([("colors", colors), ("zbuf", zbuf), ("dists", dists)], pix_to_face)
+    shape = pix_to_face.shape
+    if zbuf.shape != shape or dists.shape != shape or colors.shape != shape + (3,):
+        raise RuntimeError("pix_to_face, zbuf and dists must be (N, H, W, K) and colors (N, H, W, K, 3)")
+    if shape[3] > kMaxPointsPerPixel:
+        raise RuntimeError("Must have faces_per_pixel <= %d" % kMaxPointsPerPixel)
+    return dev
+
+
+def softmax_rgb_blend(colors: torch.Tensor, pix_to_face: torch.Tensor, zbuf: torch.Tensor, dists: torch.Tensor,
+                      sigma: float, gamma: float, background_color, znear=1.0, zfar=100.0):
+    """Fused pytorch3d.renderer.blending.softmax_rgb_blend on the rasterizer's layout (no counterpart in pytorch3d._C;
+    SURVEY.md 8f-5): colors (N,H,W,K,3) f32, pix_to_face (N,H,W,K) i64, zbuf / dists (N,H,W,K) f32; background_color a
+    float32 CUDA tensor of 3 values or 3 numbers; znear / zfar numbers or float32 (N,) CUDA tensors -> (N,H,W,4) f32."""
+    dev = _check_softmax_inputs(colors, pix_to_face, zbuf, dists)
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    bg_ptr, bg_val, zn_ptr, zf_ptr, zn, zf, keep = _softmax_side_args(dev, N, background_color, znear, zfar)
+    c, p2f, zb, dd = colors.contiguous(), pix_to_face.contiguous(), zbuf.contiguous(), dists.contiguous()
+    with torch.cuda.device(dev):
+        out = torch.empty((N, H, W, 4), dtype=torch.float32, device=dev)
+        if out.numel() == 0:
+            return out
+        _lib.check(lib.b200r_softmax_rgb_blend_forward(
+            _ptr(c), _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K, float(sigma), float(gamma), bg_ptr, bg_val, zn_ptr,
+            zf_ptr, zn, zf, _ptr(out), _stream_ptr(dev)))
+    del keep
+    return out
+
+
+def softmax_rgb_blend_backward(grad_out: torch.Tensor, colors: torch.Tensor, pix_to_face: torch.Tensor,
+                               zbuf: torch.Tensor, dists: torch.Tensor, sigma: float, gamma: float, background_color,
+                               znear=1.0, zfar=100.0):
+    """Backward of `softmax_rgb_blend` -> (grad_colors (N,H,W,K,3), grad_dists (N,H,W,K), grad_zbuf (N,H,W,K))."""
+    dev = _check_softmax_inputs(colors, pix_to_face, zbuf, dists)
+    _require_cuda(("grad_out", grad_out), ("colors", colors))
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    if grad_out.dtype != torch.float32 or tuple(grad_out.shape) != (N, H, W, 4):
+        raise RuntimeError("grad_out must be a float32 tensor of shape (N, H, W, 4)")
+    lib = _lib.load()
+    bg_ptr, bg_val, zn_ptr, zf_ptr, zn, zf, keep = _softmax_side_args(dev, N, background_color, znear, zfar)
+    go = grad_out.contiguous()
+    c, p2f, zb, dd = colors.contiguous(), pix_to_face.contiguous(), zbuf.contiguous(), dists.contiguous()
+    with torch.cuda.device(dev):
+        grad_colors = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev)
+        grad_dists = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
+        grad_zbuf = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
+        if grad_dists.numel() == 0:
+            return grad_colors, grad_dists, grad_zbuf
+        _lib.check(lib.b200r_softmax_rgb_blend_backward(
+            _ptr(go), _ptr(c), _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K, float(sigma), float(gamma), bg_ptr, bg_val,
+            zn_ptr, zf_ptr, zn, zf, _ptr(grad_colors), _ptr(grad_dists), _ptr(grad_zbuf), _stream_ptr(dev)))
+    del keep
+    return grad_colors, grad_dists, grad_zbuf
+
+
 # ------------------------------------------------------------------------------------------------ test hooks
 # pytorch3d/csrc/ext.cpp:69-73: "These are only visible for testing; users should not call them directly".  Provided so
 # that the reference's own tests of these entry points can run against this build; none of them is on the product path.

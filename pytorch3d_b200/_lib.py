@@ -16,7 +16,7 @@ if DEV_OVERRIDE:
 
 _c_f = ctypes.POINTER(ctypes.c_float)
 _vp = ctypes.c_void_p
-_i32, _i64, _f32, _sz = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_size_t
+_i32, _i64, _f32, _f64, _sz = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double, ctypes.c_size_t
 
 # name -> (restype, argtypes); mirrors include/b200_raster.h one to one.
 SIGNATURES = {
@@ -65,6 +65,14 @@ SIGNATURES = {
         ctypes.c_int, [_vp, _i64, _i64, _i64, _i64, _vp, _vp, _f32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "b200r_points_alpha_render_backward": (
         ctypes.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _f32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "b200r_sigmoid_alpha_blend_forward": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
+    "b200r_sigmoid_alpha_blend_backward": (
+        ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
+    "b200r_softmax_rgb_blend_forward": (
+        ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _vp, _vp, _vp, _vp, _f64, _f64, _vp, _vp]),
+    "b200r_softmax_rgb_blend_backward": (
+        ctypes.c_int,
+        [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _vp, _vp, _vp, _vp, _f64, _f64, _vp, _vp, _vp, _vp]),
     "b200r_interp_face_attrs_forward": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp]),
     "b200r_interp_face_attrs_backward": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "b200r_rasterize_meshes_coarse": (

@@ -11,8 +11,18 @@ and calls `_C.rasterize_meshes[_backward]`, `_C.rasterize_points[_backward]`, `_
 `pytorch3d_b200._C` for CUDA tensors and forwards everything else (including CPU tensors) to the original module,
 so `MeshRasterizer` / `PointsRasterizer` / `MeshRenderer` / `PointsRenderer` work unchanged.
 `uninstall()` restores the originals.
+
+`install_blending()` (separate, so that `install()` keeps its four modules) serves the mesh blending step:
+    pytorch3d/renderer/blending.py          from pytorch3d import _C   (sigmoid_alpha_blend[_backward])
+                                            softmax_rgb_blend, hard_rgb_blend (pure torch)
+    pytorch3d/renderer/mesh/shader.py       from ..blending import hard_rgb_blend, softmax_rgb_blend, ...
+It proxies `_C` of the blending module for the two sigmoid ops and replaces the two torch blends, in both modules, by
+functions that send float32 CUDA inputs to `pytorch3d_b200.blending` and everything else (CPU tensors, other dtypes; a
+background colour, znear or zfar that requires grad) to the originals.
 """
 import types
+
+import torch
 
 from . import _C as _b200_C
 
@@ -22,17 +32,23 @@ _OPS = ("rasterize_meshes", "rasterize_meshes_backward", "rasterize_points", "ra
         "interp_face_attrs_backward")
 _MODULES = ("pytorch3d.renderer.mesh.rasterize_meshes", "pytorch3d.renderer.points.rasterize_points",
             "pytorch3d.renderer.compositing", "pytorch3d.ops.interp_face_attrs")
+_BLEND_OPS = ("sigmoid_alpha_blend", "sigmoid_alpha_blend_backward")
+_BLEND_MODULE = "pytorch3d.renderer.blending"
+_BLEND_FUNCTIONS = ("softmax_rgb_blend", "hard_rgb_blend")
+_BLEND_FUNCTION_MODULES = ("pytorch3d.renderer.blending", "pytorch3d.renderer.mesh.shader")
 _saved = {}
+_saved_blend = {}  # (module name, attribute) -> original
 
 
 class _Proxy(types.ModuleType):
-    def __init__(self, original):
+    def __init__(self, original, ops=_OPS):
         super().__init__("pytorch3d_b200._C_proxy")
         self.__dict__["_original"] = original
+        self.__dict__["_ops"] = ops
 
     def __getattr__(self, name):
         original = self.__dict__["_original"]
-        if name in _OPS:
+        if name in self.__dict__["_ops"]:
             ours = getattr(_b200_C, name)
             theirs = getattr(original, name, None)
 
@@ -59,8 +75,56 @@ def install():
     return patched
 
 
+def _requires_grad(x):
+    return torch.is_tensor(x) and x.requires_grad
+
+
+def _float32(colors, fragments):
+    """The fused blend takes float32 colours, depths and distances; other dtypes keep the original torch code."""
+    return all(getattr(t, "dtype", None) == torch.float32
+               for t in (colors, getattr(fragments, "zbuf", None), getattr(fragments, "dists", None)))
+
+
+def _blend_dispatch(name, original):
+    from . import blending as ours
+    if name == "softmax_rgb_blend":
+        def softmax_rgb_blend(colors, fragments, blend_params, znear=1.0, zfar=100):
+            if (not colors.is_cuda or not _float32(colors, fragments)
+                    or _requires_grad(getattr(blend_params, "background_color", None))
+                    or _requires_grad(znear) or _requires_grad(zfar)):
+                return original(colors, fragments, blend_params, znear, zfar)
+            return ours.softmax_rgb_blend(colors, fragments, blend_params, znear, zfar)
+        return softmax_rgb_blend
+
+    def hard_rgb_blend(colors, fragments, blend_params):
+        if not colors.is_cuda or colors.dtype != torch.float32:
+            return original(colors, fragments, blend_params)
+        return ours.hard_rgb_blend(colors, fragments, blend_params)
+    return hard_rgb_blend
+
+
+def install_blending():
+    """Patch PyTorch3D's mesh blending (must be importable).  Returns the list of patched module names."""
+    import importlib
+    mod = importlib.import_module(_BLEND_MODULE)
+    if (_BLEND_MODULE, "_C") not in _saved_blend:
+        _saved_blend[(_BLEND_MODULE, "_C")] = mod._C
+        mod._C = _Proxy(mod._C, _BLEND_OPS)
+    for modname in _BLEND_FUNCTION_MODULES:
+        m = importlib.import_module(modname)
+        for name in _BLEND_FUNCTIONS:
+            if (modname, name) not in _saved_blend:
+                _saved_blend[(modname, name)] = getattr(m, name)
+                setattr(m, name, _blend_dispatch(name, getattr(m, name)))
+    return list(_BLEND_FUNCTION_MODULES)
+
+
 def uninstall():
+    """Undo `install()` and `install_blending()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
         del _saved[modname]
+    for (modname, name), original in list(_saved_blend.items()):
+        setattr(importlib.import_module(modname), name, original)
+        del _saved_blend[(modname, name)]
