@@ -280,6 +280,28 @@ int b200r_softmax_rgb_blend_backward(const float* grad_out, const float* colors,
                                      const float* znear, const float* zfar, double znear_value, double zfar_value,
                                      float* grad_colors, float* grad_dists, float* grad_zbuf, void* stream);
 
+/*
+ * Fused splatter blending (additional entry points, no counterpart in pytorch3d._C): what
+ * pytorch3d/renderer/splatter_blend.py SplatterBlender.forward computes after its projection step, in one kernel for
+ * the forward and two for the backward (DESIGN.md section 11).
+ *  colors float32 (N,H,W,K,3); pixel_coords_screen float32 (N,H,W,K,3) (x, y in pixels, z the depth);
+ *  background_mask bool / uint8 (N,H,W,K) (nonzero: background slot); 1 <= K <= 150; sigma > 0 in pixels.
+ *  background: device float32 (3,), or NULL and then background_value: HOST float[3].
+ *  out float32 (N,H,W,4) RGBA, fully written.
+ * Backward: grad_out float32 (N,H,W,4); workspace of b200r_splatter_blend_workspace_bytes(N, H, W) bytes, 16-byte
+ * aligned (a 96-byte record per pixel); grad_colors and grad_pixel_coords_screen float32 (N,H,W,K,3), fully written
+ * (0 in background slots and in the z channel).  No atomics: the results are deterministic.
+ */
+int b200r_splatter_blend_forward(const float* colors, const float* pixel_coords_screen, const uint8_t* background_mask,
+                                 int32_t N, int32_t H, int32_t W, int32_t K, double sigma, const float* background,
+                                 const float* background_value, float* out, void* stream);
+size_t b200r_splatter_blend_workspace_bytes(int32_t N, int32_t H, int32_t W);
+int b200r_splatter_blend_backward(const float* grad_out, const float* colors, const float* pixel_coords_screen,
+                                  const uint8_t* background_mask, int32_t N, int32_t H, int32_t W, int32_t K,
+                                  double sigma, const float* background, const float* background_value,
+                                  void* workspace, size_t workspace_bytes, float* grad_colors,
+                                  float* grad_pixel_coords_screen, void* stream);
+
 /* ------------------------------------------------------------------ frame exchange between GPUs ---------- */
 
 /*

@@ -594,15 +594,20 @@ def interp_face_attrs_backward(pix_to_face: torch.Tensor, barycentric_coords: to
     return grad_bary, grad_attrs
 
 
-def _check_blend_inputs(named_floats, pix_to_face):
-    dev = _require_cuda(*named_floats, ("pix_to_face", pix_to_face))
+_SCALAR_TYPE_NAMES = {torch.int64: "Long", torch.bool: "Bool"}
+
+
+def _check_blend_inputs(named_floats, pix_to_face, index_name="pix_to_face", index_dtype=torch.int64):
+    """float32 CUDA tensors on one device, and an (N, H, W, K) per-slot tensor `index_name` of `index_dtype` (the face
+    indices, or the splatter blend's background mask)."""
+    dev = _require_cuda(*named_floats, (index_name, pix_to_face))
     for name, t in named_floats:
         if t.dtype != torch.float32:
             raise RuntimeError("Expected tensor for %s to have scalar type Float; but got %s" % (name, t.dtype))
-    if pix_to_face.dtype != torch.int64:
-        raise RuntimeError("expected scalar type Long but found %s" % pix_to_face.dtype)
+    if pix_to_face.dtype != index_dtype:
+        raise RuntimeError("expected scalar type %s but found %s" % (_SCALAR_TYPE_NAMES[index_dtype], pix_to_face.dtype))
     if pix_to_face.dim() != 4:
-        raise RuntimeError("pix_to_face must have dimensions (N, H, W, K)")
+        raise RuntimeError("%s must have dimensions (N, H, W, K)" % index_name)
     return dev
 
 
@@ -731,6 +736,68 @@ def softmax_rgb_blend_backward(grad_out: torch.Tensor, colors: torch.Tensor, pix
             zn_ptr, zf_ptr, zn, zf, _ptr(grad_colors), _ptr(grad_dists), _ptr(grad_zbuf), _stream_ptr(dev)))
     del keep
     return grad_colors, grad_dists, grad_zbuf
+
+
+def _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma):
+    dev = _check_blend_inputs([("colors", colors), ("pixel_coords_screen", pixel_coords_screen)], background_mask,
+                              "background_mask", torch.bool)
+    shape = tuple(background_mask.shape)
+    if colors.shape != shape + (3,) or pixel_coords_screen.shape != shape + (3,):
+        raise RuntimeError("background_mask must be (N, H, W, K), colors and pixel_coords_screen (N, H, W, K, 3)")
+    if shape[3] > kMaxPointsPerPixel:
+        raise RuntimeError("Must have faces_per_pixel <= %d" % kMaxPointsPerPixel)
+    if shape[3] < 1:
+        raise RuntimeError("faces_per_pixel must be at least 1")
+    if not float(sigma) > 0.0:
+        raise RuntimeError("Only positive standard deviations make sense.")
+    return dev
+
+
+def splatter_blend(colors: torch.Tensor, pixel_coords_screen: torch.Tensor, background_mask: torch.Tensor,
+                   sigma: float, background_color):
+    """Fused splatter blend (the blend of pytorch3d.renderer.splatter_blend.SplatterBlender after its projection step;
+    no counterpart in pytorch3d._C): colors and pixel_coords_screen (N,H,W,K,3) f32, background_mask (N,H,W,K) bool,
+    sigma > 0 in pixels; background_color a float32 CUDA tensor of 3 values or 3 numbers -> (N,H,W,4) f32 RGBA."""
+    dev = _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma)
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in background_mask.shape)
+    bg_ptr, bg_val, _, _, _, _, keep = _softmax_side_args(dev, N, background_color, 1.0, 100.0)
+    c, xyz, m = colors.contiguous(), pixel_coords_screen.contiguous(), background_mask.contiguous()
+    with torch.cuda.device(dev):
+        out = torch.empty((N, H, W, 4), dtype=torch.float32, device=dev)
+        if out.numel() == 0:
+            return out
+        _lib.check(lib.b200r_splatter_blend_forward(_ptr(c), _ptr(xyz), _ptr(m), N, H, W, K, float(sigma), bg_ptr,
+                                                    bg_val, _ptr(out), _stream_ptr(dev)))
+    del keep
+    return out
+
+
+def splatter_blend_backward(grad_out: torch.Tensor, colors: torch.Tensor, pixel_coords_screen: torch.Tensor,
+                            background_mask: torch.Tensor, sigma: float, background_color):
+    """Backward of `splatter_blend` -> (grad_colors (N,H,W,K,3), grad_pixel_coords_screen (N,H,W,K,3)); both are 0 in
+    background slots, and the z channel of grad_pixel_coords_screen is 0."""
+    dev = _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma)
+    _require_cuda(("grad_out", grad_out), ("colors", colors))
+    N, H, W, K = (int(v) for v in background_mask.shape)
+    if grad_out.dtype != torch.float32 or tuple(grad_out.shape) != (N, H, W, 4):
+        raise RuntimeError("grad_out must be a float32 tensor of shape (N, H, W, 4)")
+    lib = _lib.load()
+    bg_ptr, bg_val, _, _, _, _, keep = _softmax_side_args(dev, N, background_color, 1.0, 100.0)
+    go = grad_out.contiguous()
+    c, xyz, m = colors.contiguous(), pixel_coords_screen.contiguous(), background_mask.contiguous()
+    with torch.cuda.device(dev):
+        grad_colors = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev)
+        grad_xyz = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev)
+        if grad_colors.numel() == 0:
+            return grad_colors, grad_xyz
+        ws_bytes = int(lib.b200r_splatter_blend_workspace_bytes(N, H, W))
+        workspace = torch.empty((ws_bytes // 4,), dtype=torch.float32, device=dev)  # caching allocator: 512-byte aligned
+        _lib.check(lib.b200r_splatter_blend_backward(
+            _ptr(go), _ptr(c), _ptr(xyz), _ptr(m), N, H, W, K, float(sigma), bg_ptr, bg_val, _ptr(workspace), ws_bytes,
+            _ptr(grad_colors), _ptr(grad_xyz), _stream_ptr(dev)))
+    del keep
+    return grad_colors, grad_xyz
 
 
 # ------------------------------------------------------------------------------------------------ test hooks

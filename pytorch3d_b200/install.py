@@ -19,6 +19,12 @@ so `MeshRasterizer` / `PointsRasterizer` / `MeshRenderer` / `PointsRenderer` wor
 It proxies `_C` of the blending module for the two sigmoid ops and replaces the two torch blends, in both modules, by
 functions that send float32 CUDA inputs to `pytorch3d_b200.blending` and everything else (CPU tensors, other dtypes; a
 background colour, znear or zfar that requires grad) to the originals.
+
+`install_splatter()` (separate again) serves SplatterPhongShader's blend:
+    pytorch3d/renderer/splatter_blend.py    class SplatterBlender (pure torch)
+    pytorch3d/renderer/mesh/shader.py       from ..splatter_blend import SplatterBlender
+It replaces the class name in both modules by one whose instances send float32 CUDA inputs with K <= 150 and a
+constant background colour to `pytorch3d_b200.splatter_blend`, and everything else to an instance of the original.
 """
 import types
 
@@ -36,8 +42,9 @@ _BLEND_OPS = ("sigmoid_alpha_blend", "sigmoid_alpha_blend_backward")
 _BLEND_MODULE = "pytorch3d.renderer.blending"
 _BLEND_FUNCTIONS = ("softmax_rgb_blend", "hard_rgb_blend")
 _BLEND_FUNCTION_MODULES = ("pytorch3d.renderer.blending", "pytorch3d.renderer.mesh.shader")
+_SPLATTER_MODULES = ("pytorch3d.renderer.splatter_blend", "pytorch3d.renderer.mesh.shader")
 _saved = {}
-_saved_blend = {}  # (module name, attribute) -> original
+_saved_blend = {}  # (module name, attribute) -> original (install_blending and install_splatter)
 
 
 class _Proxy(types.ModuleType):
@@ -119,8 +126,54 @@ def install_blending():
     return list(_BLEND_FUNCTION_MODULES)
 
 
+def _splatter_dispatch(original):
+    """A stand-in for the class `SplatterBlender` that sends float32 CUDA inputs with K <= 150 and a constant background
+    to the fused op, and everything else to an instance of the original class, built on first use."""
+    from . import splatter_blend as ours
+
+    class SplatterBlender(torch.nn.Module):
+        def __init__(self, input_shape, device):
+            super().__init__()
+            self._input_shape, self._device = input_shape, device
+            self._ours = ours.SplatterBlender(input_shape, device)
+            self._original = None
+
+        def to(self, device):
+            self._device = device
+            if self._original is not None:
+                self._original.to(device)
+            return super().to(device)
+
+        def forward(self, colors, pixel_coords_cameras, cameras, background_mask, blend_params):
+            if (colors.is_cuda and colors.dtype == torch.float32 and pixel_coords_cameras.dtype == torch.float32
+                    and colors.dim() == 5 and colors.shape[3] <= _b200_C.kMaxPointsPerPixel
+                    and not _requires_grad(getattr(blend_params, "background_color", None))):
+                return self._ours(colors, pixel_coords_cameras, cameras, background_mask, blend_params)
+            if self._original is None:
+                self._original = original(self._input_shape, self._device)
+            return self._original(colors, pixel_coords_cameras, cameras, background_mask, blend_params)
+
+    SplatterBlender.__qualname__ = "SplatterBlender"
+    SplatterBlender.__module__ = __name__
+    return SplatterBlender
+
+
+def install_splatter():
+    """Patch PyTorch3D's splatter blending (must be importable): the name `SplatterBlender` in
+    pytorch3d.renderer.splatter_blend and in pytorch3d.renderer.mesh.shader, where `SplatterPhongShader` builds its
+    blender.  Blenders built before the call, and names imported from those modules before it, keep the original.
+    Returns the list of patched module names."""
+    import importlib
+    for modname in _SPLATTER_MODULES:
+        m = importlib.import_module(modname)
+        if (modname, "SplatterBlender") not in _saved_blend:
+            _saved_blend[(modname, "SplatterBlender")] = m.SplatterBlender
+            m.SplatterBlender = _splatter_dispatch(m.SplatterBlender)
+    return list(_SPLATTER_MODULES)
+
+
 def uninstall():
-    """Undo `install()` and `install_blending()`."""
+    """Undo `install()`, `install_blending()` and `install_splatter()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
