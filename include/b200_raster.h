@@ -302,6 +302,42 @@ int b200r_splatter_blend_backward(const float* grad_out, const float* colors, co
                                   void* workspace, size_t workspace_bytes, float* grad_colors,
                                   float* grad_pixel_coords_screen, void* stream);
 
+/*
+ * Fused Phong / flat shading (additional entry points, no counterpart in pytorch3d._C): what
+ * pytorch3d/renderer/mesh/shading.py phong_shading, _phong_shading_with_pixels and flat_shading compute with the
+ * PointLights, DirectionalLights and AmbientLights of renderer/lighting.py, one thread per slot (DESIGN.md section 12).
+ *  pix_to_face int64 (N,H,W,K); barycentric_coords float32 (N,H,W,K,3) (phong; may be NULL when flat);
+ *  face_positions, face_normals float32 (F,3,3) (phong: corners of each face) or (F,3) (flat: centroid and normal);
+ *  face_normals may be NULL for ambient light; texels float32 (N,H,W,K,3);
+ *  params float32 (N, B200R_SHADING_PARAMS), one row per image:
+ *    [0:3] ambient (material ambient * light ambient), [3:6] light diffuse, [6:9] light specular,
+ *    [9:12] material diffuse, [12:15] material specular, [15:18] light location (point) or direction (directional),
+ *    [18:21] camera centre, [21] shininess;
+ *  light: B200R_LIGHT_POINT / _DIRECTIONAL / _AMBIENT; flat: 0 phong, 1 flat.
+ *  colors float32 (N,H,W,K,3), fully written; positions float32 (N,H,W,K,3) or NULL: the interpolated positions
+ *  (bit-identical to b200r_interp_face_attrs_forward), 0 in background slots.
+ * Backward: grad_colors float32 (N,H,W,K,3); grad_positions the same shape or NULL.  Every output may be NULL
+ *  (not computed): grad_texels, grad_barycentric_coords (N,H,W,K,3) (phong), grad_face_positions, grad_face_normals
+ *  (shapes of the face inputs; zero-filled here, then accumulated with atomics), grad_params (N, B200R_SHADING_PARAMS).
+ *  grad_params needs a workspace of b200r_shading_workspace_bytes(N, H, W, K) bytes; it and every other output except
+ *  the two face gradients are deterministic.  N <= 65535.
+ */
+#define B200R_SHADING_PARAMS 22
+#define B200R_LIGHT_POINT 0
+#define B200R_LIGHT_DIRECTIONAL 1
+#define B200R_LIGHT_AMBIENT 2
+int b200r_shading_forward(const int64_t* pix_to_face, const float* barycentric_coords, const float* face_positions,
+                          const float* face_normals, int64_t F, const float* texels, const float* params, int32_t N,
+                          int32_t H, int32_t W, int32_t K, int32_t flat, int32_t light, float* colors,
+                          float* positions, void* stream);
+size_t b200r_shading_workspace_bytes(int32_t N, int32_t H, int32_t W, int32_t K);
+int b200r_shading_backward(const float* grad_colors, const float* grad_positions, const int64_t* pix_to_face,
+                           const float* barycentric_coords, const float* face_positions, const float* face_normals,
+                           int64_t F, const float* texels, const float* params, int32_t N, int32_t H, int32_t W,
+                           int32_t K, int32_t flat, int32_t light, void* workspace, size_t workspace_bytes,
+                           float* grad_texels, float* grad_barycentric_coords, float* grad_face_positions,
+                           float* grad_face_normals, float* grad_params, void* stream);
+
 /* ------------------------------------------------------------------ frame exchange between GPUs ---------- */
 
 /*

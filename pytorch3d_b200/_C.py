@@ -800,6 +800,114 @@ def splatter_blend_backward(grad_out: torch.Tensor, colors: torch.Tensor, pixel_
     return grad_colors, grad_xyz
 
 
+SHADING_PARAMS = 22  # B200R_SHADING_PARAMS: the per-image parameter row of the shading ops
+LIGHT_KINDS = {"point": 0, "directional": 1, "ambient": 2}  # B200R_LIGHT_*
+
+
+def _check_shading_inputs(pix_to_face, barycentric_coords, face_positions, face_normals, texels, params, flat, light):
+    """The (N, H, W, K) shape; raises RuntimeError naming the argument for anything the kernels cannot take."""
+    if light not in LIGHT_KINDS:
+        raise RuntimeError("light must be one of %s, got %r" % (sorted(LIGHT_KINDS), light))
+    if light != "ambient" and face_normals is None:
+        raise RuntimeError("face_normals are required for %s light" % light)
+    if not flat and barycentric_coords is None:
+        raise RuntimeError("barycentric_coords are required for phong shading")
+    floats =[("texels", texels), ("params", params), ("face_positions", face_positions)]
+    if not flat:
+        floats.append(("barycentric_coords", barycentric_coords))
+    if light != "ambient":
+        floats.append(("face_normals", face_normals))
+    dev = _check_blend_inputs(floats, pix_to_face)
+    shape = tuple(pix_to_face.shape)
+    if tuple(texels.shape) != shape + (3,):
+        raise RuntimeError("texels must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
+                           % (tuple(texels.shape),))
+    if not flat and tuple(barycentric_coords.shape) != shape + (3,):
+        raise RuntimeError("barycentric_coords must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
+                           % (tuple(barycentric_coords.shape),))
+    face_shape = (3,) if flat else (3, 3)
+    for name, t in (("face_positions", face_positions), ("face_normals", face_normals)):
+        if t is not None and (t.dim() != 1 + len(face_shape) or tuple(t.shape[1:]) != face_shape):
+            raise RuntimeError("%s must be (F, %s), got %s"
+                               % (name, ", ".join(str(v) for v in face_shape), tuple(t.shape)))
+    if light != "ambient" and face_normals.shape[0] != face_positions.shape[0]:
+        raise RuntimeError("face_positions and face_normals must have the same number of faces")
+    if tuple(params.shape) != (shape[0], SHADING_PARAMS):
+        raise RuntimeError("params must be (N, %d), got %s" % (SHADING_PARAMS, tuple(params.shape)))
+    return dev
+
+
+def shading_forward(pix_to_face: torch.Tensor, barycentric_coords, face_positions: torch.Tensor, face_normals,
+                    texels: torch.Tensor, params: torch.Tensor, flat: bool, light: str, return_positions: bool = False):
+    """Fused Phong (flat=False) or flat shading (no counterpart in pytorch3d._C; DESIGN.md section 12): pix_to_face
+    (N,H,W,K) i64; barycentric_coords (N,H,W,K,3) f32 (phong only); face_positions / face_normals (F,3,3) f32 (phong)
+    or (F,3) (flat), face_normals unused (may be None) for ambient light; texels (N,H,W,K,3) f32; params (N,22) f32 (the
+    row of include/b200_raster.h); light "point", "directional" or "ambient".
+    -> (colors (N,H,W,K,3), positions (N,H,W,K,3) or None)."""
+    dev = _check_shading_inputs(pix_to_face, barycentric_coords, face_positions, face_normals, texels, params, flat,
+                                light)
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    F = int(face_positions.shape[0])
+    p2f, tx, prm, fp = pix_to_face.contiguous(), texels.contiguous(), params.contiguous(), face_positions.contiguous()
+    bary = None if flat else barycentric_coords.contiguous()
+    fn = None if light == "ambient" else face_normals.contiguous()
+    with torch.cuda.device(dev):
+        colors = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev)
+        positions = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev) if return_positions else None
+        if colors.numel() == 0:
+            return colors, positions
+        _lib.check(lib.b200r_shading_forward(_ptr(p2f), _ptr(bary), _ptr(fp), _ptr(fn), F, _ptr(tx), _ptr(prm), N, H,
+                                             W, K, int(bool(flat)), LIGHT_KINDS[light], _ptr(colors), _ptr(positions),
+                                             _stream_ptr(dev)))
+    return colors, positions
+
+
+def shading_backward(grad_colors: torch.Tensor, grad_positions, pix_to_face: torch.Tensor, barycentric_coords,
+                     face_positions: torch.Tensor, face_normals, texels: torch.Tensor, params: torch.Tensor, flat: bool,
+                     light: str, needs_input_grad=(True, True, True, True, True)):
+    """Backward of `shading_forward` -> (grad_texels, grad_barycentric_coords, grad_face_positions, grad_face_normals,
+    grad_params); an entry is None where `needs_input_grad` (same order) is false, and grad_barycentric_coords is None
+    in flat mode.  grad_params is deterministic; the two face gradients are accumulated with atomics."""
+    dev = _check_shading_inputs(pix_to_face, barycentric_coords, face_positions, face_normals, texels, params, flat,
+                                light)
+    shape = tuple(pix_to_face.shape) + (3,)
+    for name, t in (("grad_colors", grad_colors), ("grad_positions", grad_positions)):
+        if t is not None:
+            _require_cuda((name, t), ("pix_to_face", pix_to_face))
+            if t.dtype != torch.float32 or tuple(t.shape) != shape:
+                raise RuntimeError("%s must be a float32 tensor of shape (N, H, W, K, 3)" % name)
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    F = int(face_positions.shape[0])
+    need_tx, need_bary, need_fp, need_fn, need_prm = (bool(v) for v in needs_input_grad)
+    need_bary = need_bary and not flat
+    need_fn = need_fn and face_normals is not None
+    gc, p2f, tx, prm = grad_colors.contiguous(), pix_to_face.contiguous(), texels.contiguous(), params.contiguous()
+    gp = None if grad_positions is None else grad_positions.contiguous()
+    fp = face_positions.contiguous()
+    bary = None if flat else barycentric_coords.contiguous()
+    fn = None if light == "ambient" else face_normals.contiguous()
+    with torch.cuda.device(dev):
+        def out(flag, like_shape):
+            return torch.empty(like_shape, dtype=torch.float32, device=dev) if flag else None
+        g_tx, g_bary = out(need_tx, shape), out(need_bary, shape)
+        g_fp = out(need_fp, tuple(face_positions.shape))
+        g_fn = out(need_fn, tuple(face_normals.shape)) if need_fn else None
+        g_prm = out(need_prm, (N, SHADING_PARAMS))
+        ws_bytes = int(lib.b200r_shading_workspace_bytes(N, H, W, K)) if need_prm else 0
+        ws = torch.empty((ws_bytes // 4,), dtype=torch.float32, device=dev) if ws_bytes else None
+        _lib.check(lib.b200r_shading_backward(
+            _ptr(gc), _ptr(gp), _ptr(p2f), _ptr(bary), _ptr(fp), _ptr(fn), F, _ptr(tx), _ptr(prm), N, H, W, K,
+            int(bool(flat)), LIGHT_KINDS[light], _ptr(ws), ws_bytes, _ptr(g_tx), _ptr(g_bary), _ptr(g_fp), _ptr(g_fn),
+            _ptr(g_prm), _stream_ptr(dev)))
+        if N * H * W * K == 0:  # nothing was launched: the outputs the kernels would have written
+            for t in (g_tx, g_bary):
+                if t is not None:
+                    t.zero_()
+    return g_tx, g_bary, g_fp, g_fn, g_prm
+
+
 # ------------------------------------------------------------------------------------------------ test hooks
 # pytorch3d/csrc/ext.cpp:69-73: "These are only visible for testing; users should not call them directly".  Provided so
 # that the reference's own tests of these entry points can run against this build; none of them is on the product path.

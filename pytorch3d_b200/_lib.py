@@ -78,6 +78,13 @@ SIGNATURES = {
     "b200r_splatter_blend_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "b200r_splatter_blend_backward": (
         ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f64, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "b200r_shading_forward": (
+        ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "b200r_shading_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32]),
+    "b200r_shading_backward": (
+        ctypes.c_int,
+        [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp, _vp, _vp,
+         _vp, _vp, _vp]),
     "b200r_interp_face_attrs_forward": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp]),
     "b200r_interp_face_attrs_backward": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "b200r_rasterize_meshes_coarse": (

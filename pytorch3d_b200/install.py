@@ -25,6 +25,14 @@ background colour, znear or zfar that requires grad) to the originals.
     pytorch3d/renderer/mesh/shader.py       from ..splatter_blend import SplatterBlender
 It replaces the class name in both modules by one whose instances send float32 CUDA inputs with K <= 150 and a
 constant background colour to `pytorch3d_b200.splatter_blend`, and everything else to an instance of the original.
+
+`install_shading()` (separate again) serves the per-pixel lighting of SoftPhongShader, HardPhongShader,
+SplatterPhongShader and HardFlatShader:
+    pytorch3d/renderer/mesh/shading.py      phong_shading, _phong_shading_with_pixels, flat_shading (pure torch)
+    pytorch3d/renderer/mesh/shader.py       from .shading import _phong_shading_with_pixels, flat_shading, ...
+It replaces the three functions in both modules by functions that send float32 CUDA inputs lit by PyTorch3D's own
+PointLights / DirectionalLights / AmbientLights and Materials to `pytorch3d_b200.shading`, and everything else to the
+originals.
 """
 import types
 
@@ -43,8 +51,10 @@ _BLEND_MODULE = "pytorch3d.renderer.blending"
 _BLEND_FUNCTIONS = ("softmax_rgb_blend", "hard_rgb_blend")
 _BLEND_FUNCTION_MODULES = ("pytorch3d.renderer.blending", "pytorch3d.renderer.mesh.shader")
 _SPLATTER_MODULES = ("pytorch3d.renderer.splatter_blend", "pytorch3d.renderer.mesh.shader")
+_SHADING_MODULES = ("pytorch3d.renderer.mesh.shading", "pytorch3d.renderer.mesh.shader")
+_SHADING_FUNCTIONS = ("phong_shading", "_phong_shading_with_pixels", "flat_shading")
 _saved = {}
-_saved_blend = {}  # (module name, attribute) -> original (install_blending and install_splatter)
+_saved_blend = {}  # (module name, attribute) -> original (install_blending, install_splatter and install_shading)
 
 
 class _Proxy(types.ModuleType):
@@ -172,8 +182,66 @@ def install_splatter():
     return list(_SPLATTER_MODULES)
 
 
+def _shading_fused(fragments, lights, materials, texels):
+    """Whether the fused shading takes these inputs: float32 CUDA texels and Fragments, 3 texel channels, lights exactly
+    PyTorch3D's PointLights / DirectionalLights / AmbientLights and materials exactly its Materials, all with 3
+    channels, and material diffuse / specular colours of batch 1 (other batches do not broadcast in the reference)."""
+    import importlib
+    try:
+        lighting = importlib.import_module("pytorch3d.renderer.lighting")
+        materials_mod = importlib.import_module("pytorch3d.renderer.materials")
+    except ImportError:
+        return False
+    light_types = tuple(getattr(lighting, n) for n in ("PointLights", "DirectionalLights", "AmbientLights")
+                        if hasattr(lighting, n))
+    if type(lights) not in light_types or type(materials) is not getattr(materials_mod, "Materials", None):
+        return False
+    bary = getattr(fragments, "bary_coords", None)
+    if not (getattr(texels, "is_cuda", False) and texels.dtype == torch.float32 and texels.dim() == 5
+            and texels.shape[-1] == 3 and getattr(bary, "dtype", None) == torch.float32 and bary.is_cuda
+            and getattr(fragments.pix_to_face, "is_cuda", False) and fragments.pix_to_face.dtype == torch.int64):
+        return False
+    for owner, names in ((lights, ("ambient_color", "diffuse_color", "specular_color")),
+                         (materials, ("ambient_color", "diffuse_color", "specular_color"))):
+        for name in names:
+            t = getattr(owner, name, None)
+            if t is None and owner is lights and name != "ambient_color":
+                continue  # AmbientLights
+            if not torch.is_tensor(t) or t.dim() != 2 or t.shape[-1] != 3:
+                return False
+    return materials.diffuse_color.shape[0] == 1 and materials.specular_color.shape[0] == 1
+
+
+def _shading_dispatch(name, original):
+    from . import shading as ours
+
+    def shade(meshes, fragments, lights, cameras, materials, texels):
+        if _shading_fused(fragments, lights, materials, texels):
+            return getattr(ours, name)(meshes, fragments, lights, cameras, materials, texels)
+        return original(meshes, fragments, lights, cameras, materials, texels)
+
+    shade.__name__ = shade.__qualname__ = name
+    return shade
+
+
+def install_shading():
+    """Patch PyTorch3D's Phong and flat shading (must be importable): `phong_shading`, `_phong_shading_with_pixels` and
+    `flat_shading` in pytorch3d.renderer.mesh.shading and in pytorch3d.renderer.mesh.shader, which imports them by name.
+    Float32 CUDA inputs lit by PyTorch3D's own light and material classes go to `pytorch3d_b200.shading`; everything
+    else (CPU tensors, other dtypes, light or material subclasses with their own models) to the originals.  Returns the
+    list of patched module names."""
+    import importlib
+    for modname in _SHADING_MODULES:
+        m = importlib.import_module(modname)
+        for name in _SHADING_FUNCTIONS:
+            if (modname, name) not in _saved_blend and hasattr(m, name):
+                _saved_blend[(modname, name)] = getattr(m, name)
+                setattr(m, name, _shading_dispatch(name, getattr(m, name)))
+    return list(_SHADING_MODULES)
+
+
 def uninstall():
-    """Undo `install()`, `install_blending()` and `install_splatter()`."""
+    """Undo `install()`, `install_blending()`, `install_splatter()` and `install_shading()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original

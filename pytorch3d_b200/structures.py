@@ -54,6 +54,20 @@ class PackedMeshes:
     def isempty(self):
         return self._N == 0 or self._verts_packed.shape[0] == 0
 
+    def verts_normals_packed(self):
+        """(V, 3) unit vertex normals, as pytorch3d.structures.Meshes computes them: the sum of the area-weighted normals
+        (v2 - v1) x (v0 - v1) of the faces around each vertex, normalised with eps 1e-6.  Differentiable in the
+        vertices; computed on every call."""
+        verts, faces = self.verts_packed(), self.faces_packed()
+        if self.isempty():
+            return torch.zeros((self._N, 3), dtype=torch.int64, device=self.device)  # what Meshes returns when empty
+        corners = verts[faces]
+        face_normals = torch.cross(corners[:, 2] - corners[:, 1], corners[:, 0] - corners[:, 1], dim=1)
+        normals = torch.zeros_like(verts)
+        for j in range(3):
+            normals = normals.index_add(0, faces[:, j], face_normals)
+        return torch.nn.functional.normalize(normals, eps=1e-6, dim=1)
+
     def requires_grad_(self, flag=True):
         self._verts_packed.requires_grad_(flag)
         return self
