@@ -338,6 +338,34 @@ int b200r_shading_backward(const float* grad_colors, const float* grad_positions
                            float* grad_texels, float* grad_barycentric_coords, float* grad_face_positions,
                            float* grad_face_normals, float* grad_params, void* stream);
 
+/*
+ * Fused UV texture sampling (additional entry points, no counterpart in pytorch3d._C): what
+ * pytorch3d/renderer/mesh/textures.py TexturesUV.sample_textures computes for a texture with one map per mesh -- the
+ * slot's UV interpolated from its face's corner UVs ((0, 0) where pix_to_face < 0), mapped to grid coordinates with
+ * torch.lerp and the y flip, then F.grid_sample of map n, the slot's image -- one thread per slot (DESIGN.md section 13).
+ *  pix_to_face int64 (N,H,W,K); barycentric_coords float32 (N,H,W,K,3); face_uvs float32 (F,3,2);
+ *  maps float32 (N,H_in,W_in,C), channel last, read in place (64-bit offsets); H_in, W_in, C >= 1;
+ *  mode: B200R_SAMPLE_BILINEAR / _NEAREST; padding: B200R_PAD_ZEROS / _BORDER / _REFLECTION (torch's enum values).
+ *  texels float32 (N,H,W,K,C), fully written.
+ * Backward: grad_texels float32 (N,H,W,K,C).  Every output may be NULL (not computed): grad_maps (N,H_in,W_in,C) and
+ *  grad_face_uvs (F,3,2) are zero-filled here, then accumulated with atomics; grad_barycentric_coords (N,H,W,K,3) is
+ *  written once per slot (0 in background slots and for "nearest") and is deterministic.
+ */
+#define B200R_SAMPLE_BILINEAR 0
+#define B200R_SAMPLE_NEAREST 1
+#define B200R_PAD_ZEROS 0
+#define B200R_PAD_BORDER 1
+#define B200R_PAD_REFLECTION 2
+int b200r_texture_uv_forward(const int64_t* pix_to_face, const float* barycentric_coords, const float* face_uvs,
+                             int64_t F, const float* maps, int32_t N, int32_t H, int32_t W, int32_t K, int32_t H_in,
+                             int32_t W_in, int32_t C, int32_t mode, int32_t padding, int32_t align_corners,
+                             float* texels, void* stream);
+int b200r_texture_uv_backward(const float* grad_texels, const int64_t* pix_to_face, const float* barycentric_coords,
+                              const float* face_uvs, int64_t F, const float* maps, int32_t N, int32_t H, int32_t W,
+                              int32_t K, int32_t H_in, int32_t W_in, int32_t C, int32_t mode, int32_t padding,
+                              int32_t align_corners, float* grad_maps, float* grad_barycentric_coords,
+                              float* grad_face_uvs, void* stream);
+
 /* ------------------------------------------------------------------ frame exchange between GPUs ---------- */
 
 /*

@@ -908,6 +908,91 @@ def shading_backward(grad_colors: torch.Tensor, grad_positions, pix_to_face: tor
     return g_tx, g_bary, g_fp, g_fn, g_prm
 
 
+SAMPLING_MODES = {"bilinear": 0, "nearest": 1}  # B200R_SAMPLE_*: torch's GridSamplerInterpolation
+PADDING_MODES = {"zeros": 0, "border": 1, "reflection": 2}  # B200R_PAD_*: torch's GridSamplerPadding
+
+
+def _check_texture_inputs(pix_to_face, barycentric_coords, face_uvs, maps, sampling_mode, padding_mode):
+    """(N, H, W, K, H_in, W_in, C, device); raises RuntimeError naming the argument for anything the kernels cannot
+    take, and ValueError when the maps' batch is not the Fragments' N."""
+    if sampling_mode not in SAMPLING_MODES:
+        raise RuntimeError("sampling_mode must be one of %s, got %r" % (sorted(SAMPLING_MODES), sampling_mode))
+    if padding_mode not in PADDING_MODES:
+        raise RuntimeError("padding_mode must be one of %s, got %r" % (sorted(PADDING_MODES), padding_mode))
+    if pix_to_face.dim() != 4:
+        raise RuntimeError("pix_to_face must have dimensions (N, H, W, K)")
+    shape = tuple(pix_to_face.shape)
+    if tuple(barycentric_coords.shape) != shape + (3,):
+        raise RuntimeError("barycentric_coords must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
+                           % (tuple(barycentric_coords.shape),))
+    if face_uvs.dim() != 3 or tuple(face_uvs.shape[1:]) != (3, 2):
+        raise RuntimeError("face_uvs must be (F, 3, 2), got %s" % (tuple(face_uvs.shape),))
+    if maps.dim() != 4 or min(maps.shape[1:]) < 1:
+        raise RuntimeError("maps must be (N, H_in, W_in, C) with H_in, W_in, C >= 1, got %s" % (tuple(maps.shape),))
+    if maps.shape[0] != shape[0]:
+        raise ValueError("maps must have one map per image: maps has batch %d, the Fragments have N = %d"
+                         % (maps.shape[0], shape[0]))
+    dev = _check_blend_inputs([("barycentric_coords", barycentric_coords), ("face_uvs", face_uvs), ("maps", maps)],
+                              pix_to_face)
+    H_in, W_in, C = (int(v) for v in maps.shape[1:])
+    return shape + (H_in, W_in, C, dev)
+
+
+def texture_uv_forward(pix_to_face: torch.Tensor, barycentric_coords: torch.Tensor, face_uvs: torch.Tensor,
+                       maps: torch.Tensor, sampling_mode: str = "bilinear", padding_mode: str = "border",
+                       align_corners: bool = True):
+    """Fused TexturesUV.sample_textures for one map per image (no counterpart in pytorch3d._C; DESIGN.md section 13):
+    pix_to_face (N,H,W,K) i64, barycentric_coords (N,H,W,K,3) f32, face_uvs (F,3,2) f32, maps (N,H_in,W_in,C) f32
+    (channel last, read in place when contiguous) -> texels (N,H,W,K,C) f32, contiguous."""
+    N, H, W, K, H_in, W_in, C, dev = _check_texture_inputs(pix_to_face, barycentric_coords, face_uvs, maps,
+                                                           sampling_mode, padding_mode)
+    lib = _lib.load()
+    F = int(face_uvs.shape[0])
+    p2f, bary, fuv, m = pix_to_face.contiguous(), barycentric_coords.contiguous(), face_uvs.contiguous(), maps.contiguous()
+    with torch.cuda.device(dev):
+        texels = torch.empty((N, H, W, K, C), dtype=torch.float32, device=dev)
+        if texels.numel() == 0:
+            return texels
+        _lib.check(lib.b200r_texture_uv_forward(_ptr(p2f), _ptr(bary), _ptr(fuv), F, _ptr(m), N, H, W, K, H_in, W_in,
+                                                C, SAMPLING_MODES[sampling_mode], PADDING_MODES[padding_mode],
+                                                int(bool(align_corners)), _ptr(texels), _stream_ptr(dev)))
+    return texels
+
+
+def texture_uv_backward(grad_texels: torch.Tensor, pix_to_face: torch.Tensor, barycentric_coords: torch.Tensor,
+                        face_uvs: torch.Tensor, maps: torch.Tensor, sampling_mode: str = "bilinear",
+                        padding_mode: str = "border", align_corners: bool = True, needs_input_grad=(True, True, True)):
+    """Backward of `texture_uv_forward` -> (grad_maps (N,H_in,W_in,C), grad_barycentric_coords (N,H,W,K,3),
+    grad_face_uvs (F,3,2)); an entry is None where `needs_input_grad` (same order) is false.  grad_barycentric_coords is
+    deterministic; the other two are accumulated with atomics, so requesting them under
+    torch.use_deterministic_algorithms(True) raises, as torch's grid sampler backward does."""
+    N, H, W, K, H_in, W_in, C, dev = _check_texture_inputs(pix_to_face, barycentric_coords, face_uvs, maps,
+                                                           sampling_mode, padding_mode)
+    _require_cuda(("grad_texels", grad_texels), ("pix_to_face", pix_to_face))
+    if grad_texels.dtype != torch.float32 or tuple(grad_texels.shape) != (N, H, W, K, C):
+        raise RuntimeError("grad_texels must be a float32 tensor of shape (N, H, W, K, C) = %s, got %s %s"
+                           % ((N, H, W, K, C), grad_texels.dtype, tuple(grad_texels.shape)))
+    need_maps, need_bary, need_fuv = (bool(v) for v in needs_input_grad)
+    if ((need_maps or need_fuv) and torch.are_deterministic_algorithms_enabled()
+            and not torch.is_deterministic_algorithms_warn_only_enabled()):
+        raise RuntimeError(
+            "texture_uv_backward does not have a deterministic implementation (grad_maps and grad_face_uvs are "
+            "accumulated with atomics), but you set 'torch.use_deterministic_algorithms(True)'.")
+    lib = _lib.load()
+    F = int(face_uvs.shape[0])
+    go = grad_texels.contiguous()
+    p2f, bary, fuv, m = pix_to_face.contiguous(), barycentric_coords.contiguous(), face_uvs.contiguous(), maps.contiguous()
+    with torch.cuda.device(dev):
+        g_maps = torch.empty((N, H_in, W_in, C), dtype=torch.float32, device=dev) if need_maps else None
+        g_bary = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev) if need_bary else None
+        g_fuv = torch.empty((F, 3, 2), dtype=torch.float32, device=dev) if need_fuv else None
+        _lib.check(lib.b200r_texture_uv_backward(
+            _ptr(go), _ptr(p2f), _ptr(bary), _ptr(fuv), F, _ptr(m), N, H, W, K, H_in, W_in, C,
+            SAMPLING_MODES[sampling_mode], PADDING_MODES[padding_mode], int(bool(align_corners)), _ptr(g_maps),
+            _ptr(g_bary), _ptr(g_fuv), _stream_ptr(dev)))
+    return g_maps, g_bary, g_fuv
+
+
 # ------------------------------------------------------------------------------------------------ test hooks
 # pytorch3d/csrc/ext.cpp:69-73: "These are only visible for testing; users should not call them directly".  Provided so
 # that the reference's own tests of these entry points can run against this build; none of them is on the product path.

@@ -85,6 +85,12 @@ SIGNATURES = {
         ctypes.c_int,
         [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp, _vp, _vp,
          _vp, _vp, _vp]),
+    "b200r_texture_uv_forward": (
+        ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "b200r_texture_uv_backward": (
+        ctypes.c_int,
+        [_vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp,
+         _vp]),
     "b200r_interp_face_attrs_forward": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp]),
     "b200r_interp_face_attrs_backward": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "b200r_rasterize_meshes_coarse": (

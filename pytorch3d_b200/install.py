@@ -33,6 +33,14 @@ SplatterPhongShader and HardFlatShader:
 It replaces the three functions in both modules by functions that send float32 CUDA inputs lit by PyTorch3D's own
 PointLights / DirectionalLights / AmbientLights and Materials to `pytorch3d_b200.shading`, and everything else to the
 originals.
+
+`install_textures()` (separate again) serves the texture sampling of every mesh shader for `TexturesUV`:
+    pytorch3d/renderer/mesh/textures.py     TexturesUV.sample_textures (pure torch: interpolation, grid_sample)
+It replaces the method on the class itself, so every import path sees it.  Textures with one map per mesh (no
+`maps_ids`), float32 CUDA maps and barycentrics and int64 CUDA pix_to_face on one device, one of the two sampling modes
+"bilinear" / "nearest" and one of the three padding modes go to `pytorch3d_b200.textures`; everything else (CPU
+tensors, tensors on different devices, other dtypes, multi-map textures, "bicubic", empty textures) to the original
+method.
 """
 import types
 
@@ -53,8 +61,10 @@ _BLEND_FUNCTION_MODULES = ("pytorch3d.renderer.blending", "pytorch3d.renderer.me
 _SPLATTER_MODULES = ("pytorch3d.renderer.splatter_blend", "pytorch3d.renderer.mesh.shader")
 _SHADING_MODULES = ("pytorch3d.renderer.mesh.shading", "pytorch3d.renderer.mesh.shader")
 _SHADING_FUNCTIONS = ("phong_shading", "_phong_shading_with_pixels", "flat_shading")
+_TEXTURES_MODULE = "pytorch3d.renderer.mesh.textures"
 _saved = {}
 _saved_blend = {}  # (module name, attribute) -> original (install_blending, install_splatter and install_shading)
+_saved_methods = {}  # (module name, class name, method name) -> original (install_textures)
 
 
 class _Proxy(types.ModuleType):
@@ -240,8 +250,54 @@ def install_shading():
     return list(_SHADING_MODULES)
 
 
+def _textures_fused(textures, fragments):
+    """Whether the fused texture sampling takes this call: one map per mesh, a non-empty texture, float32 CUDA maps and
+    barycentrics and int64 CUDA pix_to_face on one device, a sampling and padding mode the kernels implement, one map per
+    image."""
+    if textures.maps_ids_padded() is not None or textures.isempty():
+        return False
+    if textures.sampling_mode not in _b200_C.SAMPLING_MODES or textures.padding_mode not in _b200_C.PADDING_MODES:
+        return False
+    maps, bary, p2f = textures.maps_padded(), getattr(fragments, "bary_coords", None), fragments.pix_to_face
+    if not all(getattr(t, "is_cuda", False) for t in (maps, bary, p2f)):
+        return False
+    if maps.device != p2f.device or bary.device != p2f.device:
+        return False  # the reference moves the maps to the Fragments' device
+    if maps.dtype != torch.float32 or bary.dtype != torch.float32 or p2f.dtype != torch.int64:
+        return False
+    return maps.dim() == 4 and p2f.dim() == 4 and maps.shape[0] == p2f.shape[0]
+
+
+def _textures_dispatch(original):
+    from . import textures as ours
+
+    def sample_textures(self, fragments, **kwargs):
+        if _textures_fused(self, fragments):
+            return ours.sample_textures(self, fragments, **kwargs)
+        return original(self, fragments, **kwargs)
+
+    sample_textures.__name__ = "sample_textures"
+    sample_textures.__qualname__ = "TexturesUV.sample_textures"
+    sample_textures.__doc__ = original.__doc__
+    return sample_textures
+
+
+def install_textures():
+    """Patch PyTorch3D's UV texture sampling (must be importable): the method `sample_textures` of the class
+    `TexturesUV` in pytorch3d.renderer.mesh.textures, so that existing objects and every import path see it.  Returns
+    the list of patched module names."""
+    import importlib
+    m = importlib.import_module(_TEXTURES_MODULE)
+    key = (_TEXTURES_MODULE, "TexturesUV", "sample_textures")
+    if key not in _saved_methods:
+        cls = m.TexturesUV
+        _saved_methods[key] = cls.__dict__["sample_textures"]
+        cls.sample_textures = _textures_dispatch(cls.__dict__["sample_textures"])
+    return [_TEXTURES_MODULE]
+
+
 def uninstall():
-    """Undo `install()`, `install_blending()`, `install_splatter()` and `install_shading()`."""
+    """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()` and `install_textures()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
@@ -249,3 +305,6 @@ def uninstall():
     for (modname, name), original in list(_saved_blend.items()):
         setattr(importlib.import_module(modname), name, original)
         del _saved_blend[(modname, name)]
+    for (modname, clsname, name), original in list(_saved_methods.items()):
+        setattr(getattr(importlib.import_module(modname), clsname), name, original)
+        del _saved_methods[(modname, clsname, name)]

@@ -64,6 +64,35 @@ def torus_batch(n_meshes: int, rings: int, sides: int, seed: int = 0, device="cp
     return PackedMeshes(vs, fs)
 
 
+def torus_uvs(rings: int, sides: int):
+    """UVs of `torus(rings, sides)` from its (ring, side) parametrisation: (verts_uvs ((rings+1)*(sides+1), 2) f32,
+    faces_uvs (F, 3) i64), faces in the order of `torus`.  The UV grid has one more row and column than the vertex grid,
+    so the vertices on the two seams are duplicated in UV space and `faces_uvs` differs from `faces` there."""
+    uu, vv = torch.meshgrid(torch.arange(rings + 1, dtype=torch.float64) / rings,
+                            torch.arange(sides + 1, dtype=torch.float64) / sides, indexing="ij")
+    verts_uvs = torch.stack([uu, vv], -1).reshape(-1, 2).to(torch.float32)
+    S = sides + 1
+    i = torch.arange(rings).reshape(-1, 1)
+    j = torch.arange(sides).reshape(1, -1)
+    a = (i * S + j).reshape(-1)
+    b = ((i + 1) * S + j).reshape(-1)
+    c = ((i + 1) * S + j + 1).reshape(-1)
+    d = (i * S + j + 1).reshape(-1)
+    faces_uvs = torch.cat([torch.stack([a, b, c], 1), torch.stack([a, c, d], 1)], 0).to(torch.int64)
+    return verts_uvs, faces_uvs
+
+
+def textured_torus_batch(n_meshes: int, rings: int, sides: int, map_size=(64, 64), channels: int = 3, seed: int = 0,
+                         device="cpu"):
+    """`torus_batch` with UV texture coordinates and maps: (meshes, verts_uvs list of (V_uv, 2), faces_uvs list of
+    (F, 3), maps (n_meshes, H_in, W_in, channels) f32 in [0, 1), one seeded map per mesh)."""
+    meshes = torus_batch(n_meshes, rings, sides, seed=seed, device=device)
+    verts_uvs, faces_uvs = torus_uvs(rings, sides)
+    gen = torch.Generator().manual_seed(seed + 1)
+    maps = torch.rand((n_meshes, int(map_size[0]), int(map_size[1]), channels), generator=gen).to(device)
+    return meshes, [verts_uvs.to(device)] * n_meshes, [faces_uvs.to(device)] * n_meshes, maps
+
+
 def torus_batch_hetero(face_counts, seed: int = 0, device="cpu"):
     """Batch of tori whose face counts approximate `face_counts` (rings = sides = sqrt(F/2))."""
     gen = torch.Generator().manual_seed(seed)
