@@ -366,6 +366,49 @@ int b200r_texture_uv_backward(const float* grad_texels, const int64_t* pix_to_fa
                               int32_t align_corners, float* grad_maps, float* grad_barycentric_coords,
                               float* grad_face_uvs, void* stream);
 
+/*
+ * Fused frustum culling and z-clipping (additional entry points, no counterpart in pytorch3d._C): what
+ * pytorch3d/renderer/mesh/clip.py clip_faces and convert_clipped_rasterization_to_original_faces compute, with the
+ * reference's output layout (DESIGN.md section 14).  All entry points are asynchronous.
+ *  Frustum: planes[6] = left, right, top, bottom, znear, zfar (host array, float32); bit i of cull_mask says plane i is
+ *  used (0 when the frustum does not cull).  has_z_clip / z_clip: the clipping plane (compared and subtracted as
+ *  float32, divided by as a multiply by (float)(1.0 / z_clip), as torch's CUDA kernels do).
+ *  Count: face_verts float32 (F,3,3), or (face_verts NULL) verts float32 (V,3) with faces int64 (F,3) read in place.
+ *  workspace: b200r_clip_faces_workspace_words(F) int64 words; words 0..3 become the record {F_clipped, n_case3,
+ *  n_case4, number of faces culled or clipped}, which the caller reads to size the outputs of the fill.
+ *  Fill: the same face_verts and frustum as the count, and its workspace.  Outputs face_verts_clipped (F_clipped,3,3),
+ *  first_clipped / num_clipped (N,), clipped_to_unclipped (F_clipped,); when n_case3 + n_case4 > 0 also
+ *  barycentric_conversion (n_case3 + 2 n_case4,3,3), clipped_to_conversion and neighbor_idx (F_clipped,).
+ *  Backward: grad_face_verts (F,3,3) written once per face from grad_face_verts_clipped and grad_conversion (each may be
+ *  NULL: no gradient); deterministic.
+ *  Convert: pix_to_face int64 and barycentric_coords float32 of S slots; barycentric_coords_unclipped may be NULL (then
+ *  only pix_to_face is mapped).  Convert backward: grad_conversion (T,3,3) is zero-filled here and accumulated with
+ *  atomics; grad_barycentric_coords is written once per slot; either may be NULL.
+ */
+int64_t b200r_clip_faces_workspace_words(int64_t F);
+int b200r_clip_faces_count(const float* face_verts, const float* verts, const int64_t* faces, int64_t F,
+                           const float* planes, int32_t cull_mask, int32_t has_z_clip, double z_clip,
+                           int64_t* workspace, void* stream);
+int b200r_clip_faces_fill(const float* face_verts, int64_t F, const int64_t* mesh_to_face_first_idx, int32_t N,
+                          const float* planes, int32_t cull_mask, int32_t has_z_clip, double z_clip,
+                          int32_t perspective_correct, const int64_t* workspace, int64_t F_clipped, int64_t n_case3,
+                          int64_t n_case4, float* face_verts_clipped, int64_t* first_clipped, int64_t* num_clipped,
+                          int64_t* clipped_to_unclipped, float* barycentric_conversion,
+                          int64_t* clipped_to_conversion, int64_t* neighbor_idx, void* stream);
+int b200r_clip_faces_backward(const float* face_verts, int64_t F, const float* planes, int32_t cull_mask,
+                              int32_t has_z_clip, double z_clip, int32_t perspective_correct,
+                              const int64_t* workspace, int64_t n_case3, int64_t n_case4,
+                              const float* grad_face_verts_clipped, const float* grad_conversion,
+                              float* grad_face_verts, void* stream);
+int b200r_clip_convert_forward(const int64_t* pix_to_face, const float* barycentric_coords, int64_t S,
+                               const int64_t* clipped_to_unclipped, const float* barycentric_conversion,
+                               const int64_t* clipped_to_conversion, int64_t* pix_to_face_unclipped,
+                               float* barycentric_coords_unclipped, void* stream);
+int b200r_clip_convert_backward(const float* grad_barycentric_coords_unclipped, const int64_t* pix_to_face,
+                                const float* barycentric_coords, int64_t S, const float* barycentric_conversion,
+                                const int64_t* clipped_to_conversion, int64_t T, float* grad_barycentric_coords,
+                                float* grad_conversion, void* stream);
+
 /* ------------------------------------------------------------------ frame exchange between GPUs ---------- */
 
 /*

@@ -11,6 +11,7 @@ uses) or, for the ops it does not cover, through ctypes.  PyTorch is used only f
 There is no CPU path: CPU tensors raise RuntimeError, like a CUDA-less build of the reference does
 for CUDA tensors (rasterize_meshes.h:137-139, mirrored).
 """
+import ctypes
 from typing import Tuple
 
 import torch
@@ -991,6 +992,176 @@ def texture_uv_backward(grad_texels: torch.Tensor, pix_to_face: torch.Tensor, ba
             SAMPLING_MODES[sampling_mode], PADDING_MODES[padding_mode], int(bool(align_corners)), _ptr(g_maps),
             _ptr(g_bary), _ptr(g_fuv), _stream_ptr(dev)))
     return g_maps, g_bary, g_fuv
+
+
+def _clip_frustum_args(frustum):
+    """(planes (6,) float32 host array, cull_mask, has_z_clip, z_clip, perspective_correct) of a ClipFrustum-like
+    object for the b200r_clip_* entry points."""
+    values = (frustum.left, frustum.right, frustum.top, frustum.bottom, frustum.znear, frustum.zfar)
+    mask = 0
+    if frustum.cull:
+        for i, v in enumerate(values):
+            if v is not None:
+                mask |= 1 << i
+    planes = (ctypes.c_float * 6)(*[0.0 if v is None else float(v) for v in values])
+    z = frustum.z_clip_value
+    return planes, mask, int(z is not None), 0.0 if z is None else float(z), int(bool(frustum.perspective_correct))
+
+
+def _check_face_verts(face_verts):
+    if face_verts.dtype != torch.float32 or face_verts.dim() != 3 or tuple(face_verts.shape[1:]) != (3, 3):
+        raise RuntimeError("face_verts must be a float32 tensor of shape (F, 3, 3), got %s %s"
+                           % (face_verts.dtype, tuple(face_verts.shape)))
+
+
+def clip_faces_count(frustum, face_verts=None, verts=None, faces=None):
+    """Count pass of the fused clip_faces (DESIGN.md section 14): classifies every face of face_verts (F,3,3) -- or of
+    verts[faces], read in place -- against `frustum` and returns the int64 workspace whose first four words are the
+    record (F_clipped, n_case3, n_case4, number of faces culled or clipped).  Asynchronous: the caller reads the record."""
+    if face_verts is not None:
+        _check_face_verts(face_verts)
+        dev = _require_cuda(("face_verts", face_verts))
+        F = int(face_verts.shape[0])
+        fv, v, f = face_verts.contiguous(), None, None
+    else:
+        if verts.dtype != torch.float32 or verts.dim() != 2 or verts.shape[1] != 3:
+            raise RuntimeError("verts must be a float32 tensor of shape (V, 3), got %s %s"
+                               % (verts.dtype, tuple(verts.shape)))
+        if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
+            raise RuntimeError("faces must be an int64 tensor of shape (F, 3), got %s %s"
+                               % (faces.dtype, tuple(faces.shape)))
+        dev = _require_cuda(("verts", verts), ("faces", faces))
+        F = int(faces.shape[0])
+        fv, v, f = None, verts.contiguous(), faces.contiguous()
+    lib = _lib.load()
+    planes, mask, has_z, z, _ = _clip_frustum_args(frustum)
+    with torch.cuda.device(dev):
+        ws = torch.empty((int(lib.b200r_clip_faces_workspace_words(F)),), dtype=torch.int64, device=dev)
+        _lib.check(lib.b200r_clip_faces_count(_ptr(fv), _ptr(v), _ptr(f), F, planes, mask, has_z, z, _ptr(ws),
+                                              _stream_ptr(dev)))
+    return ws
+
+
+def _check_clip_ranges(face_verts, mesh_to_face_first_idx, num_faces_per_mesh):
+    for name, t in (("mesh_to_face_first_idx", mesh_to_face_first_idx), ("num_faces_per_mesh", num_faces_per_mesh)):
+        if t.dtype != torch.int64 or t.dim() != 1:
+            raise RuntimeError("%s must be an int64 tensor of shape (N,), got %s %s" % (name, t.dtype, tuple(t.shape)))
+    if num_faces_per_mesh.shape[0] != mesh_to_face_first_idx.shape[0]:
+        raise RuntimeError("num_faces_per_mesh must have the same size as mesh_to_face_first_idx")
+    return _require_cuda(("face_verts", face_verts), ("mesh_to_face_first_idx", mesh_to_face_first_idx),
+                         ("num_faces_per_mesh", num_faces_per_mesh))
+
+
+def clip_faces_fill(face_verts, mesh_to_face_first_idx, num_faces_per_mesh, frustum, workspace, record):
+    """Fill pass of the fused clip_faces: the seven ClippedFaces fields in the reference's layout, from the workspace of
+    `clip_faces_count(frustum, face_verts)` and its record (a 4-sequence read by the caller).  The last three are empty
+    tensors when no face was clipped (only culled)."""
+    _check_face_verts(face_verts)
+    dev = _check_clip_ranges(face_verts, mesh_to_face_first_idx, num_faces_per_mesh)
+    lib = _lib.load()
+    F, N = int(face_verts.shape[0]), int(mesh_to_face_first_idx.shape[0])
+    F_clipped, n3, n4 = (int(v) for v in record[:3])
+    T = n3 + 2 * n4
+    planes, mask, has_z, z, persp = _clip_frustum_args(frustum)
+    fv, first = face_verts.contiguous(), mesh_to_face_first_idx.contiguous()
+    with torch.cuda.device(dev):
+        out_fv = torch.empty((F_clipped, 3, 3), dtype=torch.float32, device=dev)
+        out_first = torch.empty((N,), dtype=torch.int64, device=dev)
+        out_num = torch.empty((N,), dtype=torch.int64, device=dev)
+        c2u = torch.empty((F_clipped,), dtype=torch.int64, device=dev)
+        conv = torch.empty((T, 3, 3), dtype=torch.float32, device=dev)
+        conv_idx = torch.empty((F_clipped if T > 0 else 0,), dtype=torch.int64, device=dev)
+        neighbor = torch.empty((F_clipped if T > 0 else 0,), dtype=torch.int64, device=dev)
+        _lib.check(lib.b200r_clip_faces_fill(
+            _ptr(fv), F, _ptr(first), N, planes, mask, has_z, z, persp, _ptr(workspace), F_clipped, n3, n4,
+            _ptr(out_fv), _ptr(out_first), _ptr(out_num), _ptr(c2u), _ptr(conv), _ptr(conv_idx), _ptr(neighbor),
+            _stream_ptr(dev)))
+    return out_fv, out_first, out_num, c2u, conv, conv_idx, neighbor
+
+
+def clip_faces_backward(face_verts, frustum, workspace, record, grad_face_verts_clipped, grad_conversion):
+    """d loss / d face_verts (F,3,3) of the fused clip_faces from the gradients of its clipped face_verts and of its
+    barycentric_conversion (either may be None); deterministic, no host synchronisation."""
+    _check_face_verts(face_verts)
+    dev = _require_cuda(("face_verts", face_verts), ("workspace", workspace))
+    n3, n4 = int(record[1]), int(record[2])
+    for name, g in (("grad_face_verts_clipped", grad_face_verts_clipped), ("grad_conversion", grad_conversion)):
+        if g is not None:
+            _require_cuda(("face_verts", face_verts), (name, g))
+            if g.dtype != torch.float32:
+                raise RuntimeError("%s must be float32, got %s" % (name, g.dtype))
+    lib = _lib.load()
+    F = int(face_verts.shape[0])
+    planes, mask, has_z, z, persp = _clip_frustum_args(frustum)
+    fv = face_verts.contiguous()
+    gfv = grad_face_verts_clipped.contiguous() if grad_face_verts_clipped is not None else None
+    gc = grad_conversion.contiguous() if grad_conversion is not None else None
+    with torch.cuda.device(dev):
+        grad = torch.empty((F, 3, 3), dtype=torch.float32, device=dev)
+        _lib.check(lib.b200r_clip_faces_backward(_ptr(fv), F, planes, mask, has_z, z, persp, _ptr(workspace), n3, n4,
+                                                 _ptr(gfv), _ptr(gc), _ptr(grad), _stream_ptr(dev)))
+    return grad
+
+
+def clip_convert_forward(pix_to_face, barycentric_coords, faces_clipped_to_unclipped_idx, barycentric_conversion=None,
+                         faces_clipped_to_conversion_idx=None):
+    """Fused convert_clipped_rasterization_to_original_faces: (pix_to_face_unclipped, bary_unclipped).  Without a
+    conversion only pix_to_face is mapped and bary_unclipped is None."""
+    if pix_to_face.dtype != torch.int64:
+        raise RuntimeError("pix_to_face must be int64, got %s" % pix_to_face.dtype)
+    if barycentric_coords.dtype != torch.float32 or tuple(barycentric_coords.shape) != tuple(pix_to_face.shape) + (3,):
+        raise RuntimeError("barycentric_coords must be a float32 tensor of shape pix_to_face.shape + (3,), got %s %s"
+                           % (barycentric_coords.dtype, tuple(barycentric_coords.shape)))
+    named = [("pix_to_face", pix_to_face), ("barycentric_coords", barycentric_coords),
+             ("faces_clipped_to_unclipped_idx", faces_clipped_to_unclipped_idx)]
+    if barycentric_conversion is not None:
+        if barycentric_conversion.dtype != torch.float32 or tuple(barycentric_conversion.shape[1:]) != (3, 3):
+            raise RuntimeError("barycentric_conversion must be a float32 tensor of shape (T, 3, 3), got %s %s"
+                               % (barycentric_conversion.dtype, tuple(barycentric_conversion.shape)))
+        named += [("barycentric_conversion", barycentric_conversion),
+                  ("faces_clipped_to_conversion_idx", faces_clipped_to_conversion_idx)]
+    dev = _require_cuda(*named)
+    lib = _lib.load()
+    p2f, bary = pix_to_face.contiguous(), barycentric_coords.contiguous()
+    c2u = faces_clipped_to_unclipped_idx.contiguous()
+    conv = barycentric_conversion.contiguous() if barycentric_conversion is not None else None
+    cidx = faces_clipped_to_conversion_idx.contiguous() if barycentric_conversion is not None else None
+    with torch.cuda.device(dev):
+        p2f_out = torch.empty_like(p2f)
+        bary_out = torch.empty_like(bary) if conv is not None else None
+        _lib.check(lib.b200r_clip_convert_forward(_ptr(p2f), _ptr(bary), p2f.numel(), _ptr(c2u), _ptr(conv),
+                                                  _ptr(cidx), _ptr(p2f_out), _ptr(bary_out), _stream_ptr(dev)))
+    return p2f_out, bary_out
+
+
+def clip_convert_backward(grad_bary_unclipped, pix_to_face, barycentric_coords, barycentric_conversion,
+                          faces_clipped_to_conversion_idx, needs_input_grad=(True, True)):
+    """Backward of `clip_convert_forward` -> (grad_barycentric_coords, grad_conversion); an entry is None where
+    `needs_input_grad` (same order) is false.  grad_conversion is accumulated with atomics, so requesting it under
+    torch.use_deterministic_algorithms(True) raises, like the rasterizer backward in the same graph."""
+    dev = _require_cuda(("grad_bary_unclipped", grad_bary_unclipped), ("pix_to_face", pix_to_face),
+                        ("barycentric_coords", barycentric_coords), ("barycentric_conversion", barycentric_conversion),
+                        ("faces_clipped_to_conversion_idx", faces_clipped_to_conversion_idx))
+    if grad_bary_unclipped.dtype != torch.float32 or grad_bary_unclipped.shape != barycentric_coords.shape:
+        raise RuntimeError("grad_bary_unclipped must be a float32 tensor of shape %s, got %s %s"
+                           % (tuple(barycentric_coords.shape), grad_bary_unclipped.dtype,
+                              tuple(grad_bary_unclipped.shape)))
+    need_bary, need_conv = (bool(v) for v in needs_input_grad)
+    if need_conv and torch.are_deterministic_algorithms_enabled() and \
+            not torch.is_deterministic_algorithms_warn_only_enabled():
+        raise RuntimeError(
+            "clip_convert_backward does not have a deterministic implementation (grad_conversion is accumulated with "
+            "atomics), but you set 'torch.use_deterministic_algorithms(True)'.")
+    lib = _lib.load()
+    g, p2f, bary = grad_bary_unclipped.contiguous(), pix_to_face.contiguous(), barycentric_coords.contiguous()
+    conv, cidx = barycentric_conversion.contiguous(), faces_clipped_to_conversion_idx.contiguous()
+    T = int(conv.shape[0])
+    with torch.cuda.device(dev):
+        g_bary = torch.empty_like(bary) if need_bary else None
+        g_conv = torch.empty_like(conv) if need_conv else None
+        _lib.check(lib.b200r_clip_convert_backward(_ptr(g), _ptr(p2f), _ptr(bary), p2f.numel(), _ptr(conv), _ptr(cidx),
+                                                   T, _ptr(g_bary), _ptr(g_conv), _stream_ptr(dev)))
+    return g_bary, g_conv
 
 
 # ------------------------------------------------------------------------------------------------ test hooks

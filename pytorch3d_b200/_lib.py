@@ -91,7 +91,17 @@ SIGNATURES = {
         ctypes.c_int,
         [_vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp,
          _vp]),
-    "b200r_interp_face_attrs_forward": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp]),
+    "b200r_clip_faces_workspace_words": (_i64, [_i64]),
+    "b200r_clip_faces_count": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i32, _i32, _f64, _vp, _vp]),
+    "b200r_clip_faces_fill": (
+        ctypes.c_int,
+        [_vp, _i64, _vp, _i32, _vp, _i32, _i32, _f64, _i32, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+         _vp]),
+    "b200r_clip_faces_backward": (
+        ctypes.c_int, [_vp, _i64, _vp, _i32, _i32, _f64, _i32, _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "b200r_clip_convert_forward": (ctypes.c_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200r_clip_convert_backward": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp]),
+    "b200r_interp_face_attrs_forward":(ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp]),
     "b200r_interp_face_attrs_backward": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "b200r_rasterize_meshes_coarse": (
         ctypes.c_int, [_vp, _i64, _vp, _vp, _i32, _i32, _i32, _f32, _i32, _i32, _vp, _vp, _vp, _vp]),

@@ -24,6 +24,8 @@ from typing import Optional, Tuple
 
 import torch
 
+from . import _C
+
 
 class ClippedFaces:
     """Clipped faces plus what is needed to map rasterization results back to the unclipped faces
@@ -235,3 +237,93 @@ def convert_clipped_rasterization_to_original_faces(pix_to_face_clipped, bary_co
     bary_unclipped = bary_coords_clipped.clone()
     bary_unclipped[mask] = converted
     return pix_to_face_unclipped, bary_unclipped
+
+
+# ------------------------------------------------------------------------------------------ fused (CUDA) versions
+# The same two steps on the GPU kernels of csrc/clip.cu (DESIGN.md section 14), with the reference's output layout:
+# barycentric_conversion has one row per clipped face that needs one -- case-3 faces, then the first and then the
+# second halves of case-4 faces -- and faces_clipped_to_conversion_idx points into it.  The host reads one four-word
+# record per forward call (output sizes, and whether anything was culled or clipped at all); nothing else synchronises.
+
+class _ClipFacesFused(torch.autograd.Function):
+    """Fill pass and its backward; differentiable outputs: face_verts and barycentric_conversion."""
+
+    @staticmethod
+    def forward(ctx, face_verts, mesh_to_face_first_idx, num_faces_per_mesh, frustum, workspace, record):
+        outs = _C.clip_faces_fill(face_verts, mesh_to_face_first_idx, num_faces_per_mesh, frustum, workspace, record)
+        ctx.save_for_backward(face_verts, workspace)
+        ctx.frustum, ctx.record = frustum, tuple(record)
+        ctx.mark_non_differentiable(outs[1], outs[2], outs[3], outs[5], outs[6])
+        ctx.set_materialize_grads(False)
+        return outs
+
+    @staticmethod
+    def backward(ctx, grad_face_verts, _g1, _g2, _g3, grad_conversion, _g5, _g6):
+        face_verts, workspace = ctx.saved_tensors
+        grad = None
+        if ctx.needs_input_grad[0] and (grad_face_verts is not None or grad_conversion is not None):
+            grad = _C.clip_faces_backward(face_verts, ctx.frustum, workspace, ctx.record, grad_face_verts,
+                                          grad_conversion)
+        return grad, None, None, None, None, None
+
+
+def _clip_faces_counted(face_verts, mesh_to_face_first_idx, num_faces_per_mesh, frustum, workspace, record):
+    """clip_faces_fused after its count pass; `record` is the workspace's first four words, read by the caller."""
+    F_clipped, n3, n4, changed = (int(v) for v in record)
+    if changed == 0:  # nothing culled or clipped: the reference returns its inputs (clip.py:384-389)
+        return ClippedFaces(face_verts=face_verts, mesh_to_face_first_idx=mesh_to_face_first_idx,
+                            num_faces_per_mesh=num_faces_per_mesh)
+    fv, first, num, c2u, conv, conv_idx, neighbor = _ClipFacesFused.apply(
+        face_verts, mesh_to_face_first_idx, num_faces_per_mesh, frustum, workspace, record)
+    if n3 + n4 == 0:  # only culled (clip.py:465-471)
+        return ClippedFaces(face_verts=fv, mesh_to_face_first_idx=first, num_faces_per_mesh=num,
+                            faces_clipped_to_unclipped_idx=c2u)
+    return ClippedFaces(face_verts=fv, mesh_to_face_first_idx=first, num_faces_per_mesh=num,
+                        faces_clipped_to_unclipped_idx=c2u, barycentric_conversion=conv,
+                        faces_clipped_to_conversion_idx=conv_idx, clipped_faces_neighbor_idx=neighbor)
+
+
+def clip_faces_fused(face_verts_unclipped: torch.Tensor, mesh_to_face_first_idx: torch.Tensor,
+                     num_faces_per_mesh: torch.Tensor, frustum: ClipFrustum) -> ClippedFaces:
+    """`clip_faces` on the GPU for float32 CUDA tensors, in the reference's layout (a drop-in for
+    pytorch3d.renderer.mesh.clip.clip_faces).  Differentiable w.r.t. face_verts_unclipped through the clipped
+    face_verts and barycentric_conversion.  One host synchronisation: the read of the count pass's record."""
+    workspace = _C.clip_faces_count(frustum, face_verts=face_verts_unclipped)
+    record = workspace[:4].tolist()
+    return _clip_faces_counted(face_verts_unclipped, mesh_to_face_first_idx, num_faces_per_mesh, frustum, workspace,
+                               record)
+
+
+class _ConvertClippedFused(torch.autograd.Function):
+    """Barycentric conversion of a rasterization of clipped faces; differentiable w.r.t. bary and the conversion."""
+
+    @staticmethod
+    def forward(ctx, pix_to_face, bary, conversion, c2u, conv_idx):
+        p2f, bary_u = _C.clip_convert_forward(pix_to_face, bary, c2u, conversion, conv_idx)
+        ctx.save_for_backward(pix_to_face, bary, conversion, conv_idx)
+        ctx.mark_non_differentiable(p2f)
+        ctx.set_materialize_grads(False)
+        return p2f, bary_u
+
+    @staticmethod
+    def backward(ctx, _grad_p2f, grad_bary):
+        pix_to_face, bary, conversion, conv_idx = ctx.saved_tensors
+        need = (ctx.needs_input_grad[1], ctx.needs_input_grad[2])
+        if grad_bary is None or not any(need):
+            return None, None, None, None, None
+        g_bary, g_conv = _C.clip_convert_backward(grad_bary, pix_to_face, bary, conversion, conv_idx, need)
+        return None, g_bary, g_conv, None, None
+
+
+def convert_clipped_fused(pix_to_face_clipped: torch.Tensor, bary_coords_clipped: torch.Tensor,
+                          clipped_faces) -> Tuple[torch.Tensor, torch.Tensor]:
+    """`convert_clipped_rasterization_to_original_faces` on the GPU, for any ClippedFaces in the reference's layout
+    (from clip_faces_fused or from the reference's own clip_faces).  No host synchronisation."""
+    c2u = clipped_faces.faces_clipped_to_unclipped_idx
+    if c2u is None or c2u.numel() == 0:
+        return pix_to_face_clipped, bary_coords_clipped
+    conversion = clipped_faces.barycentric_conversion
+    if conversion is None:
+        return _C.clip_convert_forward(pix_to_face_clipped, bary_coords_clipped, c2u)[0], bary_coords_clipped
+    return _ConvertClippedFused.apply(pix_to_face_clipped, bary_coords_clipped, conversion, c2u,
+                                      clipped_faces.faces_clipped_to_conversion_idx)

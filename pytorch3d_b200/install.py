@@ -41,7 +41,15 @@ It replaces the method on the class itself, so every import path sees it.  Textu
 "bilinear" / "nearest" and one of the three padding modes go to `pytorch3d_b200.textures`; everything else (CPU
 tensors, tensors on different devices, other dtypes, multi-map textures, "bicubic", empty textures) to the original
 method.
+
+`install_clipping()` (separate again) serves the frustum culling and z-clipping that `MeshRasterizer` turns on for
+perspective cameras:
+    pytorch3d/renderer/mesh/rasterize_meshes.py   from .clip import clip_faces, convert_clipped_rasterization_to_...
+It replaces the two names in that module by functions that send float32 CUDA face_verts (and the Fragments of such a
+call) to `pytorch3d_b200.clip`'s fused pair, returning the reference's own `ClippedFaces`; everything else (CPU
+tensors, other dtypes) goes to the originals.
 """
+import importlib
 import types
 
 import torch
@@ -62,8 +70,11 @@ _SPLATTER_MODULES = ("pytorch3d.renderer.splatter_blend", "pytorch3d.renderer.me
 _SHADING_MODULES = ("pytorch3d.renderer.mesh.shading", "pytorch3d.renderer.mesh.shader")
 _SHADING_FUNCTIONS = ("phong_shading", "_phong_shading_with_pixels", "flat_shading")
 _TEXTURES_MODULE = "pytorch3d.renderer.mesh.textures"
+_CLIP_MODULE = "pytorch3d.renderer.mesh.rasterize_meshes"
+_CLIP_FUNCTIONS = ("clip_faces", "convert_clipped_rasterization_to_original_faces")
 _saved = {}
-_saved_blend = {}  # (module name, attribute) -> original (install_blending, install_splatter and install_shading)
+# (module name, attribute) -> original (install_blending, install_splatter, install_shading and install_clipping)
+_saved_blend = {}
 _saved_methods = {}  # (module name, class name, method name) -> original (install_textures)
 
 
@@ -296,8 +307,46 @@ def install_textures():
     return [_TEXTURES_MODULE]
 
 
+def _clip_dispatch(name, original):
+    from . import clip as ours
+
+    if name == "clip_faces":
+        def clip_faces(face_verts_unclipped, mesh_to_face_first_idx, num_faces_per_mesh, frustum):
+            if not (getattr(face_verts_unclipped, "is_cuda", False) and face_verts_unclipped.dtype == torch.float32):
+                return original(face_verts_unclipped, mesh_to_face_first_idx, num_faces_per_mesh, frustum)
+            out = ours.clip_faces_fused(face_verts_unclipped, mesh_to_face_first_idx, num_faces_per_mesh, frustum)
+            cls = importlib.import_module("pytorch3d.renderer.mesh.clip").ClippedFaces
+            return cls(**{f: getattr(out, f) for f in ours.ClippedFaces.__slots__})
+
+        return clip_faces
+
+    def convert_clipped_rasterization_to_original_faces(pix_to_face_clipped, bary_coords_clipped, clipped_faces):
+        conv = getattr(clipped_faces, "barycentric_conversion", None)
+        if not (getattr(pix_to_face_clipped, "is_cuda", False) and pix_to_face_clipped.dtype == torch.int64
+                and getattr(bary_coords_clipped, "dtype", None) == torch.float32
+                and (conv is None or conv.dtype == torch.float32)):
+            return original(pix_to_face_clipped, bary_coords_clipped, clipped_faces)
+        return ours.convert_clipped_fused(pix_to_face_clipped, bary_coords_clipped, clipped_faces)
+
+    return convert_clipped_rasterization_to_original_faces
+
+
+def install_clipping():
+    """Patch PyTorch3D's frustum culling and z-clipping (must be importable): `clip_faces` and
+    `convert_clipped_rasterization_to_original_faces` in pytorch3d.renderer.mesh.rasterize_meshes, which imports them
+    by name.  Float32 CUDA inputs go to the fused functions of `pytorch3d_b200.clip`; everything else to the originals.
+    Returns the list of patched module names."""
+    m = importlib.import_module(_CLIP_MODULE)
+    for name in _CLIP_FUNCTIONS:
+        if (_CLIP_MODULE, name) not in _saved_blend:
+            _saved_blend[(_CLIP_MODULE, name)] = getattr(m, name)
+            setattr(m, name, _clip_dispatch(name, getattr(m, name)))
+    return [_CLIP_MODULE]
+
+
 def uninstall():
-    """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()` and `install_textures()`."""
+    """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_textures()` and
+    `install_clipping()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original

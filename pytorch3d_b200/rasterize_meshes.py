@@ -9,7 +9,8 @@ import numpy as np
 import torch
 
 from . import _C
-from .clip import ClipFrustum, clip_faces, convert_clipped_rasterization_to_original_faces
+from .clip import (ClipFrustum, _clip_faces_counted, clip_faces, convert_clipped_fused,
+                   convert_clipped_rasterization_to_original_faces)
 
 # kMaxItemsPerBin (rasterization_utils.cuh:50); mirrored by rasterize_meshes.py:24-27 of the reference
 kMaxFacesPerBin = 22
@@ -83,10 +84,25 @@ def rasterize_meshes(
 
     # Cull faces outside the view frustum and clip faces that are partially behind the camera to
     # z >= z_clip_value; this may change the number of faces (rasterize_meshes.py:160-183 of the reference)
-    face_verts = verts_packed[faces_packed]
     frustum = ClipFrustum(left=-1, right=1, top=-1, bottom=1, perspective_correct=perspective_correct,
                           z_clip_value=z_clip_value, cull=cull_to_frustum)
-    clipped_faces = clip_faces(face_verts, mesh_to_face_first_idx, num_faces_per_mesh, frustum=frustum)
+    fused = verts_packed.is_cuda and verts_packed.dtype == torch.float32
+    if fused:
+        # count pass on verts[faces] in place; its record is the forward's one host read
+        workspace = _C.clip_faces_count(frustum, verts=verts_packed, faces=faces_packed)
+        record = workspace[:4].tolist()
+        if record[3] == 0:
+            # nothing culled or clipped: clip_faces would return its input unchanged, so the fused gather path
+            # computes the same Fragments without materialising face_verts
+            return _RasterizeMeshesIndexed.apply(
+                verts_packed, faces_packed, mesh_to_face_first_idx, num_faces_per_mesh, im_size, blur_radius,
+                faces_per_pixel, perspective_correct, clip_barycentric_coords, cull_backfaces)
+        face_verts = verts_packed[faces_packed]
+        clipped_faces = _clip_faces_counted(face_verts, mesh_to_face_first_idx, num_faces_per_mesh, frustum,
+                                            workspace, record)
+    else:
+        face_verts = verts_packed[faces_packed]
+        clipped_faces = clip_faces(face_verts, mesh_to_face_first_idx, num_faces_per_mesh, frustum=frustum)
     face_verts = clipped_faces.face_verts
     mesh_to_face_first_idx = clipped_faces.mesh_to_face_first_idx
     num_faces_per_mesh = clipped_faces.num_faces_per_mesh
@@ -103,8 +119,8 @@ def rasterize_meshes(
 
     # express face indices and barycentrics in terms of the original, unclipped faces
     # (rasterize_meshes.py:239-249 of the reference)
-    pix_to_face, barycentric_coords = convert_clipped_rasterization_to_original_faces(
-        pix_to_face, barycentric_coords, clipped_faces)
+    convert = convert_clipped_fused if fused else convert_clipped_rasterization_to_original_faces
+    pix_to_face, barycentric_coords = convert(pix_to_face, barycentric_coords, clipped_faces)
     return pix_to_face, zbuf, barycentric_coords, dists
 
 
