@@ -367,6 +367,29 @@ int b200r_texture_uv_backward(const float* grad_texels, const int64_t* pix_to_fa
                               float* grad_face_uvs, void* stream);
 
 /*
+ * Fused texture atlas sampling (additional entry points, no counterpart in pytorch3d._C): what
+ * pytorch3d/renderer/mesh/textures.py TexturesAtlas.sample_textures computes -- the slot's cell of its face's R x R
+ * patch from (b0, b1) with the reference's truncation, clamp and diagonal flip, read with torch's negative-index wrap
+ * and multiplied by float(pix_to_face >= 0) -- one thread per slot (DESIGN.md section 15).
+ *  pix_to_face int64 (N,H,W,K); barycentric_coords float32 (N,H,W,K,3); atlas float32 (F,R,R,C), contiguous, read in
+ *  place (64-bit offsets); R, C >= 1.  texels float32 (N,H,W,K,C), fully written.  A slot whose cell the reference
+ *  cannot index (it raises) gets texel 0.
+ * Backward: grad_texels float32 (N,H,W,K,C) -> grad_atlas float32 (F,R,R,C), zero-filled here, then every cell that
+ *  receives a contribution is written once: the sum of its slots' grad_texels * float(pix_to_face >= 0) in ascending
+ *  slot order from +0.  Deterministic, no atomics (a stable radix sort of (cell, slot) pairs).  N*H*W*K < 2^31.
+ *  workspace: b200r_texture_atlas_workspace_bytes(N, H, W, K, F, R) bytes, a function of the shapes only (0 when there
+ *  is nothing to sort or no device to size the sort for).
+ */
+size_t b200r_texture_atlas_workspace_bytes(int32_t N, int32_t H, int32_t W, int32_t K, int64_t F, int32_t R);
+int b200r_texture_atlas_forward(const int64_t* pix_to_face, const float* barycentric_coords, const float* atlas,
+                                int64_t F, int32_t R, int32_t C, int32_t N, int32_t H, int32_t W, int32_t K,
+                                float* texels, void* stream);
+int b200r_texture_atlas_backward(const float* grad_texels, const int64_t* pix_to_face,
+                                 const float* barycentric_coords, int64_t F, int32_t R, int32_t C, int32_t N,
+                                 int32_t H, int32_t W, int32_t K, void* workspace, size_t workspace_bytes,
+                                 float* grad_atlas, void* stream);
+
+/*
  * Fused frustum culling and z-clipping (additional entry points, no counterpart in pytorch3d._C): what
  * pytorch3d/renderer/mesh/clip.py clip_faces and convert_clipped_rasterization_to_original_faces compute, with the
  * reference's output layout (DESIGN.md section 14).  All entry points are asynchronous.

@@ -994,6 +994,65 @@ def texture_uv_backward(grad_texels: torch.Tensor, pix_to_face: torch.Tensor, ba
     return g_maps, g_bary, g_fuv
 
 
+def texture_atlas_key_bits(F: int, R: int):
+    """(key bits, key bytes) of the backward's sort for an (F, R, R, C) atlas: the cells and the sentinel F·R² need
+    ceil(log2(F·R² + 1)) bits; keys are 32-bit below 2³² cells and 64-bit from there (b200r_texture_atlas_backward)."""
+    bits = max(1, (int(F) * int(R) * int(R)).bit_length())
+    return bits, 4 if bits <= 32 else 8
+
+
+def _check_atlas_inputs(pix_to_face, barycentric_coords, atlas):
+    """(N, H, W, K, F, R, C, device); raises RuntimeError naming the argument for anything the kernels cannot take."""
+    if pix_to_face.dim() != 4:
+        raise RuntimeError("pix_to_face must have dimensions (N, H, W, K)")
+    shape = tuple(pix_to_face.shape)
+    if tuple(barycentric_coords.shape) != shape + (3,):
+        raise RuntimeError("barycentric_coords must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
+                           % (tuple(barycentric_coords.shape),))
+    if atlas.dim() != 4 or atlas.shape[1] != atlas.shape[2] or atlas.shape[1] < 1 or atlas.shape[3] < 1:
+        raise RuntimeError("atlas must be (F, R, R, C) with R, C >= 1, got %s" % (tuple(atlas.shape),))
+    dev = _check_blend_inputs([("barycentric_coords", barycentric_coords), ("atlas", atlas)], pix_to_face)
+    F, R, _, C = (int(v) for v in atlas.shape)
+    return shape + (F, R, C, dev)
+
+
+def texture_atlas_forward(pix_to_face: torch.Tensor, barycentric_coords: torch.Tensor, atlas: torch.Tensor):
+    """Fused TexturesAtlas.sample_textures (no counterpart in pytorch3d._C; DESIGN.md section 15): pix_to_face
+    (N,H,W,K) i64, barycentric_coords (N,H,W,K,3) f32, atlas (F,R,R,C) f32, the packed atlas (read in place when
+    contiguous) -> texels (N,H,W,K,C) f32, contiguous.  Slots whose cell the reference cannot index (it raises) get 0."""
+    N, H, W, K, F, R, C, dev = _check_atlas_inputs(pix_to_face, barycentric_coords, atlas)
+    lib = _lib.load()
+    p2f, bary, a = pix_to_face.contiguous(), barycentric_coords.contiguous(), atlas.contiguous()
+    with torch.cuda.device(dev):
+        texels = torch.empty((N, H, W, K, C), dtype=torch.float32, device=dev)
+        if texels.numel() == 0:
+            return texels
+        _lib.check(lib.b200r_texture_atlas_forward(_ptr(p2f), _ptr(bary), _ptr(a), F, R, C, N, H, W, K, _ptr(texels),
+                                                   _stream_ptr(dev)))
+    return texels
+
+
+def texture_atlas_backward(grad_texels: torch.Tensor, pix_to_face: torch.Tensor, barycentric_coords: torch.Tensor,
+                           atlas: torch.Tensor):
+    """Backward of `texture_atlas_forward` -> grad_atlas (F,R,R,C) f32: each cell's sum of grad_texels ·
+    float(pix_to_face >= 0) over the slots that read it, in ascending slot order.  Deterministic (a stable sort, no
+    atomics), so it runs under torch.use_deterministic_algorithms(True); nothing synchronises the host."""
+    N, H, W, K, F, R, C, dev = _check_atlas_inputs(pix_to_face, barycentric_coords, atlas)
+    _require_cuda(("grad_texels", grad_texels), ("pix_to_face", pix_to_face))
+    if grad_texels.dtype != torch.float32 or tuple(grad_texels.shape) != (N, H, W, K, C):
+        raise RuntimeError("grad_texels must be a float32 tensor of shape (N, H, W, K, C) = %s, got %s %s"
+                           % ((N, H, W, K, C), grad_texels.dtype, tuple(grad_texels.shape)))
+    lib = _lib.load()
+    go, p2f, bary = grad_texels.contiguous(), pix_to_face.contiguous(), barycentric_coords.contiguous()
+    with torch.cuda.device(dev):
+        grad_atlas = torch.empty((F, R, R, C), dtype=torch.float32, device=dev)
+        ws_bytes = int(lib.b200r_texture_atlas_workspace_bytes(N, H, W, K, F, R))
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None  # 512-byte aligned
+        _lib.check(lib.b200r_texture_atlas_backward(_ptr(go), _ptr(p2f), _ptr(bary), F, R, C, N, H, W, K, _ptr(ws),
+                                                    ws_bytes, _ptr(grad_atlas), _stream_ptr(dev)))
+    return grad_atlas
+
+
 def _clip_frustum_args(frustum):
     """(planes (6,) float32 host array, cull_mask, has_z_clip, z_clip, perspective_correct) of a ClipFrustum-like
     object for the b200r_clip_* entry points."""

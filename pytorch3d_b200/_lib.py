@@ -91,6 +91,11 @@ SIGNATURES = {
         ctypes.c_int,
         [_vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp,
          _vp]),
+    "b200r_texture_atlas_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i64, _i32]),
+    "b200r_texture_atlas_forward": (
+        ctypes.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "b200r_texture_atlas_backward": (
+        ctypes.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp, _vp]),
     "b200r_clip_faces_workspace_words": (_i64, [_i64]),
     "b200r_clip_faces_count": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i32, _i32, _f64, _vp, _vp]),
     "b200r_clip_faces_fill": (

@@ -42,6 +42,13 @@ It replaces the method on the class itself, so every import path sees it.  Textu
 tensors, tensors on different devices, other dtypes, multi-map textures, "bicubic", empty textures) to the original
 method.
 
+`install_texture_atlas()` (separate again) serves the texture sampling of every mesh shader for `TexturesAtlas`:
+    pytorch3d/renderer/mesh/textures.py     TexturesAtlas.sample_textures (pure torch: a dozen elementwise ops, a gather)
+It replaces the method on the class itself, as `install_textures()` does.  It packs the atlas once; a non-empty float32
+CUDA atlas (F, R, R, C) with R >= 1, int64 CUDA pix_to_face and float32 barycentrics on one device go to
+`pytorch3d_b200.texture_atlas`; everything else (CPU tensors, tensors on different devices, other dtypes, empty
+textures) to the original method.
+
 `install_clipping()` (separate again) serves the frustum culling and z-clipping that `MeshRasterizer` turns on for
 perspective cameras:
     pytorch3d/renderer/mesh/rasterize_meshes.py   from .clip import clip_faces, convert_clipped_rasterization_to_...
@@ -75,7 +82,7 @@ _CLIP_FUNCTIONS = ("clip_faces", "convert_clipped_rasterization_to_original_face
 _saved = {}
 # (module name, attribute) -> original (install_blending, install_splatter, install_shading and install_clipping)
 _saved_blend = {}
-_saved_methods = {}  # (module name, class name, method name) -> original (install_textures)
+_saved_methods = {}  # (module name, class name, method name) -> original (install_textures, install_texture_atlas)
 
 
 class _Proxy(types.ModuleType):
@@ -307,6 +314,47 @@ def install_textures():
     return [_TEXTURES_MODULE]
 
 
+def _atlas_fused(atlas, fragments):
+    """Whether the fused atlas sampling takes this call: a float32 CUDA atlas (F, R, R, C) with R >= 1 (an empty texture
+    packs to R = 0), float32 barycentrics and int64 CUDA pix_to_face, all on one device."""
+    bary, p2f = getattr(fragments, "bary_coords", None), fragments.pix_to_face
+    if not all(getattr(t, "is_cuda", False) for t in (atlas, bary, p2f)):
+        return False
+    if atlas.device != p2f.device or bary.device != p2f.device:
+        return False
+    if atlas.dtype != torch.float32 or bary.dtype != torch.float32 or p2f.dtype != torch.int64:
+        return False
+    return atlas.dim() == 4 and atlas.shape[1] >= 1 and p2f.dim() == 4
+
+
+def _atlas_dispatch(original):
+    from . import texture_atlas as ours
+
+    def sample_textures(self, fragments, **kwargs):
+        atlas = self.atlas_packed()  # once: the fused path samples this very tensor
+        if _atlas_fused(atlas, fragments):
+            return ours.sample_textures_atlas(fragments, atlas)
+        return original(self, fragments, **kwargs)
+
+    sample_textures.__name__ = "sample_textures"
+    sample_textures.__qualname__ = "TexturesAtlas.sample_textures"
+    sample_textures.__doc__ = original.__doc__
+    return sample_textures
+
+
+def install_texture_atlas():
+    """Patch PyTorch3D's texture atlas sampling (must be importable): the method `sample_textures` of the class
+    `TexturesAtlas` in pytorch3d.renderer.mesh.textures, so that existing objects and every import path see it.
+    Returns the list of patched module names."""
+    m = importlib.import_module(_TEXTURES_MODULE)
+    key = (_TEXTURES_MODULE, "TexturesAtlas", "sample_textures")
+    if key not in _saved_methods:
+        cls = m.TexturesAtlas
+        _saved_methods[key] = cls.__dict__["sample_textures"]
+        cls.sample_textures = _atlas_dispatch(cls.__dict__["sample_textures"])
+    return [_TEXTURES_MODULE]
+
+
 def _clip_dispatch(name, original):
     from . import clip as ours
 
@@ -345,8 +393,8 @@ def install_clipping():
 
 
 def uninstall():
-    """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_textures()` and
-    `install_clipping()`."""
+    """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_textures()`,
+    `install_texture_atlas()` and `install_clipping()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
