@@ -8,11 +8,6 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "lib", "libb200raster.so")
-# development: B200R_LIB=<path> runs everything against another build of the library (through the ctypes binding:
-# the torch extension is linked against the in-tree library)
-DEV_OVERRIDE = os.environ.get("B200R_LIB")
-if DEV_OVERRIDE:
-    LIB_PATH = os.path.abspath(DEV_OVERRIDE)
 
 _c_f = ctypes.POINTER(ctypes.c_float)
 _vp = ctypes.c_void_p

@@ -1,6 +1,7 @@
-"""Builds pytorch3d_b200/lib/libb200raster.so (hand-written sm_90a kernels + C ABI) with nvcc.
+"""Builds pytorch3d_b200/lib/libb200raster.so (hand-written sm_90a kernels + C ABI) with nvcc, and the torch C++
+extension over it (csrc/torch_ext.cpp) with g++.
 
-nvcc cross-compiles without a GPU; the built .so is git-ignored.
+nvcc cross-compiles without a GPU; the built .so files are git-ignored.
 Usage: python -m pytorch3d_b200.build [--force] [--verbose]
 """
 import os
@@ -33,8 +34,14 @@ def is_stale():
 
 
 def build(force=False, verbose=False):
-    if not force and not is_stale():
-        return LIB
+    """libb200raster.so, then the torch extension over it, each rebuilt when stale; returns the library's path."""
+    if force or is_stale():
+        _build_lib(verbose)
+    _build_ext(force, verbose)
+    return LIB
+
+
+def _build_lib(verbose):
     os.makedirs(LIB_DIR, exist_ok=True)
     cmd = [_nvcc(), "-O3", "-std=c++17"] + ARCH_FLAGS + ["-lineinfo",
            "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v", "-o", LIB] + [os.path.join(CSRC, f) for f in SOURCES]
@@ -45,7 +52,6 @@ def build(force=False, verbose=False):
         print(res.stdout)
     if res.returncode != 0:
         raise RuntimeError("nvcc failed building libb200raster.so (see output above)")
-    return LIB
 
 
 EXT_NAME = "_b200_ext"
@@ -57,11 +63,11 @@ def ext_path():
     return os.path.join(LIB_DIR, EXT_NAME + (sysconfig.get_config_var("EXT_SUFFIX") or ".so"))
 
 
-def build_ext(force=False, verbose=False):
-    """The torch C++ extension over the C ABI (csrc/torch_ext.cpp): what `pytorch3d_b200._C` binds to, like
-    `pytorch3d._C` in the reference (ext.cpp, setup.py:143-151).  Plain g++ with torch's own include / library paths
-    (the same the reference's setup.py passes through torch.utils.cpp_extension); links libb200raster.so by $ORIGIN."""
-    build(force=force, verbose=verbose)
+def _build_ext(force, verbose):
+    """The torch C++ extension over the C ABI (csrc/torch_ext.cpp): what `pytorch3d_b200._C` binds the rasterizer ops
+    to, like `pytorch3d._C` in the reference (ext.cpp, setup.py:143-151).  Plain g++ with torch's own include / library
+    paths (the same the reference's setup.py passes through torch.utils.cpp_extension); links libb200raster.so by
+    $ORIGIN."""
     out = ext_path()
     deps = [EXT_SRC, os.path.join(HERE, "..", "include", "b200_raster.h")]
     if not force and os.path.exists(out) and all(os.path.getmtime(d) <= os.path.getmtime(out) for d in deps):
@@ -94,4 +100,4 @@ def build_ext(force=False, verbose=False):
 if __name__ == "__main__":
     build(force="--force" in sys.argv, verbose=True)
     print("built", LIB)
-    print("built", build_ext(force="--force" in sys.argv, verbose=True))
+    print("built", ext_path())

@@ -51,7 +51,7 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> rasterize_meshes(
     const c10::optional<at::Tensor>& clipped_faces_neighbor_idx, const std::tuple<int, int> image_size,
     const double blur_radius, const int64_t faces_per_pixel, const int64_t bin_size, const int64_t max_faces_per_bin,
     const bool perspective_correct, const bool clip_barycentric_coords, const bool cull_backfaces,
-    const int64_t pair_capacity) {
+    const int64_t pair_capacity, const bool neighbors_all_minus_one) {
   TORCH_CHECK(face_verts.dim() == 3 && face_verts.size(1) == 3 && face_verts.size(2) == 3,
               "face_verts must have dimensions (num_faces, 3, 3)");
   TORCH_CHECK(num_faces_per_mesh.size(0) == mesh_to_face_first_idx.size(0),
@@ -78,8 +78,11 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> rasterize_meshes(
   const at::Tensor fv = face_verts.contiguous();
   const at::Tensor first = mesh_to_face_first_idx.contiguous().to(at::kLong);
   const at::Tensor num = num_faces_per_mesh.contiguous().to(at::kLong);
+  // A neighbour tensor the caller knows to be all -1 is checked like any other but not passed on: NULL selects the
+  // kernel variant without the clipped-face neighbour logic.
   at::Tensor nb;
-  if (clipped_faces_neighbor_idx.has_value() && F > 0) nb = clipped_faces_neighbor_idx->contiguous().to(at::kLong);
+  if (clipped_faces_neighbor_idx.has_value() && !neighbors_all_minus_one && F > 0)
+    nb = clipped_faces_neighbor_idx->contiguous().to(at::kLong);
   const auto fopt = fv.options();
   at::Tensor pix_to_face = at::empty({N, H, W, K}, fopt.dtype(at::kLong));
   at::Tensor zbuf = at::empty({N, H, W, K}, fopt);
@@ -273,7 +276,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("num_faces_per_mesh"), py::arg("clipped_faces_neighbor_idx"), py::arg("image_size"),
         py::arg("blur_radius"), py::arg("faces_per_pixel"), py::arg("bin_size"), py::arg("max_faces_per_bin"),
         py::arg("perspective_correct"), py::arg("clip_barycentric_coords"), py::arg("cull_backfaces"),
-        py::arg("pair_capacity") = 0);
+        py::arg("pair_capacity") = 0, py::arg("neighbors_all_minus_one") = false);
   m.def("rasterize_meshes_backward", &rasterize_meshes_backward);
   m.def("rasterize_meshes_indexed", &rasterize_meshes_indexed, py::arg("verts_packed"), py::arg("faces_packed"),
         py::arg("mesh_to_face_first_idx"), py::arg("num_faces_per_mesh"), py::arg("image_size"),

@@ -58,15 +58,13 @@ def test_sass_contains_tma_bulk_copy(built_lib):
     assert "sm_90a" in sass or "SM90" in sass.upper() or "EF_CUDA_SM90" in sass
 
 
-def test_torch_extension_binding_loads_and_mirrors_the_reference_ops(built_lib):
+def test_torch_extension_loads_and_mirrors_the_reference_ops(built_lib):
     """csrc/torch_ext.cpp: the pybind11 / torch C++ extension over the C ABI (the binding pytorch3d/csrc/ext.cpp:53-56
     is for the reference) is built next to the library, loads on a CPU-only machine and exports the four ops of the path
     (+ the fused indexed pair); like a CUDA-less build of the reference it raises RuntimeError for CPU tensors."""
     import pytest
     import torch
-    from pytorch3d_b200 import _C, build
-    build.build_ext()
-    assert _C.binding() == "torch-extension"
+    from pytorch3d_b200 import _C
     ext = _C._ext()
     for name in ("rasterize_meshes", "rasterize_meshes_backward", "rasterize_points", "rasterize_points_backward",
                  "rasterize_meshes_indexed", "rasterize_meshes_backward_indexed"):
@@ -81,3 +79,29 @@ def test_torch_extension_binding_loads_and_mirrors_the_reference_ops(built_lib):
     with pytest.raises(RuntimeError, match="Must have points_per_pixel <= 150"):
         ext.rasterize_meshes(fv, torch.zeros(1, dtype=torch.int64), torch.tensor([2]), None, (8, 8), 0.0, 151, 0, 0,
                              False, False, False)
+
+
+def test_missing_torch_extension_raises_import_error(built_lib, monkeypatch, tmp_path):
+    """The rasterizer ops have one binding: without the torch extension they fail loudly with the build command, and
+    never fall back to another binding."""
+    import pytest
+    import torch
+    from pytorch3d_b200 import _C, build
+    monkeypatch.setattr(build, "ext_path", lambda: str(tmp_path / "missing_ext.so"))
+    monkeypatch.setattr(_C, "_EXT", None)  # forget an extension loaded by an earlier test
+    with pytest.raises(ImportError, match=r"python -m pytorch3d_b200\.build"):
+        _C.rasterize_meshes(torch.zeros(2, 3, 3), torch.zeros(1, dtype=torch.int64), torch.tensor([2]),
+                            torch.full((2,), -1), (8, 8), 0.0, 2, 0, 0, False, False, False)
+
+
+def test_tagged_neighbour_tensor_is_still_checked(built_lib):
+    """A clipped_faces_neighbor_idx tagged as all -1 only selects the kernel variant; the extension checks its length
+    like that of an untagged one."""
+    import pytest
+    import torch
+    from pytorch3d_b200 import _C
+    z = torch.zeros(1, dtype=torch.int64)
+    nb = torch.full((3,), -1, dtype=torch.int64)
+    nb._b200_all_minus_one = True
+    with pytest.raises(RuntimeError, match="clipped_faces_neighbor_idx must have save size first dimension"):
+        _C.rasterize_meshes(torch.zeros(4, 3, 3), z, z, nb, (8, 8), 0.0, 1, 0, 0, False, False, False)

@@ -282,44 +282,31 @@ def test_blur_and_k16_north_star_variants(ops, dev):
                                  max_tie_pixels=2e-2)
 
 
-def test_both_bindings_of_the_c_abi_agree(ops, dev):
-    """The hot ops through the torch C++ extension (csrc/torch_ext.cpp, the default) and through ctypes: same library,
-    same kernels -- forward outputs bit-identical, gradients equal up to the order of the atomic additions; and the
+def test_torch_extension_binding_of_the_c_abi(ops, dev):
+    """The hot ops through their one binding, the torch C++ extension (csrc/torch_ext.cpp): forward and backward run for
+    meshes and points, a neighbour tensor tagged all -1 gives the same pix_to_face as the plain all -1 tensor, and the
     extension's error behaviour mirrors the reference ops (RuntimeError)."""
-    from pytorch3d_b200 import build
-    build.build_ext()
-    assert ops.binding() == "torch-extension", "the torch extension must be the binding in use on a GPU"
     fv, first, num = rand_faces(3000, 2, seed=3)
     fv, first, num = fv.to(dev), first.to(dev), num.to(dev)
     pts, pfirst, pnum, rad = (t.to(dev) for t in rand_points(4000, 2, seed=5))
     nb_plain = _minus_one(fv.shape[0], dev, tagged=False)
-    results = {}
-    for use_ext in (True, False):
-        ops.USE_EXT = use_ext
-        try:
-            assert ops.binding() == ("torch-extension" if use_ext else "ctypes")
-            out = {}
-            for name, nb in (("tagged", _minus_one(fv.shape[0], dev)), ("plain", nb_plain)):
-                f = ops.rasterize_meshes(fv, first, num, nb, (48, 64), 1e-3, 5, 0, 0, True, True, False)
-                g = upstream([tuple(t.shape) for t in f[1:]])
-                out[name] = (f, ops.rasterize_meshes_backward(fv, f[0], g[0].to(dev), g[1].to(dev), g[2].to(dev), True,
-                                                              True))
-            p = ops.rasterize_points(pts, pfirst, pnum, (40, 56), rad, 6, 0, 0)
-            gp = upstream([tuple(t.shape) for t in p[1:]])
-            out["points"] = (p, ops.rasterize_points_backward(pts, p[0], gp[0].to(dev), gp[1].to(dev)))
-            results[use_ext] = out
-            with pytest.raises(RuntimeError, match="face_verts must have dimensions"):
-                ops.rasterize_meshes(fv[:, :2], first, num, nb_plain, (8, 8), 0.0, 2, 0, 0, False, False, False)
-            with pytest.raises(RuntimeError, match="CUDA tensor"):
-                ops.rasterize_points(pts.cpu(), pfirst, pnum, (8, 8), rad, 2, 0, 0)
-        finally:
-            ops.USE_EXT = True
+    out = {}
+    for name, nb in (("tagged", _minus_one(fv.shape[0], dev)), ("plain", nb_plain)):
+        f = ops.rasterize_meshes(fv, first, num, nb, (48, 64), 1e-3, 5, 0, 0, True, True, False)
+        g = upstream([tuple(t.shape) for t in f[1:]])
+        out[name] = (f, ops.rasterize_meshes_backward(fv, f[0], g[0].to(dev), g[1].to(dev), g[2].to(dev), True, True))
+    p = ops.rasterize_points(pts, pfirst, pnum, (40, 56), rad, 6, 0, 0)
+    gp = upstream([tuple(t.shape) for t in p[1:]])
+    out["points"] = (p, ops.rasterize_points_backward(pts, p[0], gp[0].to(dev), gp[1].to(dev)))
+    with pytest.raises(RuntimeError, match="face_verts must have dimensions"):
+        ops.rasterize_meshes(fv[:, :2], first, num, nb_plain, (8, 8), 0.0, 2, 0, 0, False, False, False)
+    with pytest.raises(RuntimeError, match="CUDA tensor"):
+        ops.rasterize_points(pts.cpu(), pfirst, pnum, (8, 8), rad, 2, 0, 0)
     for key in ("tagged", "plain", "points"):
-        (fa, ga), (fb, gb) = results[True][key], results[False][key]
-        for a, b in zip(fa, fb):
-            assert a.dtype == b.dtype and a.shape == b.shape and torch.equal(a, b), key
-        assert torch.allclose(ga, gb, rtol=1e-4, atol=1e-5), key
-    assert torch.equal(results[True]["tagged"][0][0], results[True]["plain"][0][0])
+        (frags, grad), want_grad_shape = out[key], ((fv.shape[0], 3, 3) if key != "points" else (pts.shape[0], 3))
+        assert (frags[0] >= 0).any(), key
+        assert grad.shape == want_grad_shape and not grad.isnan().any() and (grad != 0).any(), key
+    assert torch.equal(out["tagged"][0][0], out["plain"][0][0])
 
 
 COARSE_CASES = [((64, 64), 16, 0.0), ((48, 80), 8, 1e-3), ((33, 47), 16, 1e-2)]
