@@ -339,6 +339,38 @@ int b200r_shading_backward(const float* grad_colors, const float* grad_positions
                            float* grad_face_normals, float* grad_params, void* stream);
 
 /*
+ * Fused Gouraud shading (additional entry points, no counterpart in pytorch3d._C): what
+ * pytorch3d/renderer/mesh/shading.py gouraud_shading computes -- every vertex lit with its mesh's parameter row, the
+ * shaded vertex colours then interpolated at the rasterized slots (DESIGN.md section 16).
+ *  verts, normals, verts_colors float32 (V,3) packed; normals may be NULL for ambient light;
+ *  mesh_first_vert, mesh_num_verts int64 (meshes,) device arrays: mesh m owns vertices [first[m], first[m] + num[m]);
+ *  the ranges must cover every vertex once (the packed layout; the vertex outputs are written over the ranges only),
+ *  and V > 0 needs meshes > 0;
+ *  params float32 (meshes, B200R_SHADING_PARAMS), one row per mesh in the layout above; faces int64 (F,3) packed;
+ *  pix_to_face int64 (P,) and barycentric_coords float32 (P,3) with P = N*H*W*K; light: B200R_LIGHT_*.
+ *  verts_shaded float32 (V,3) and colors float32 (P,3), fully written; colors are bit-identical to
+ *  b200r_interp_face_attrs_forward fed verts_shaded[faces].  meshes <= 65535.
+ * Backward: grad_colors float32 (P,3); verts_shaded as returned by the forward.  Every output may be NULL: grad_verts,
+ *  grad_normals, grad_verts_colors (V,3), grad_barycentric_coords (P,3), grad_params (meshes, B200R_SHADING_PARAMS).
+ *  Any of the vertex-side outputs (all but grad_barycentric_coords) needs a workspace of
+ *  b200r_gouraud_workspace_bytes(meshes, V) bytes.  grad_barycentric_coords is bit-identical to
+ *  b200r_interp_face_attrs_backward's; the vertex-side gradients start from a sum accumulated with atomics.
+ */
+int b200r_gouraud_forward(const float* verts, const float* normals, const float* verts_colors, int64_t V,
+                          const int64_t* mesh_first_vert, const int64_t* mesh_num_verts, int32_t meshes,
+                          const float* params, const int64_t* faces, int64_t F, const int64_t* pix_to_face,
+                          const float* barycentric_coords, int64_t P, int32_t light, float* verts_shaded,
+                          float* colors, void* stream);
+size_t b200r_gouraud_workspace_bytes(int32_t meshes, int64_t V);
+int b200r_gouraud_backward(const float* grad_colors, const float* verts, const float* normals,
+                           const float* verts_colors, int64_t V, const int64_t* mesh_first_vert,
+                           const int64_t* mesh_num_verts, int32_t meshes, const float* params, const int64_t* faces,
+                           int64_t F, const int64_t* pix_to_face, const float* barycentric_coords, int64_t P,
+                           int32_t light, const float* verts_shaded, void* workspace, size_t workspace_bytes,
+                           float* grad_verts, float* grad_normals, float* grad_verts_colors,
+                           float* grad_barycentric_coords, float* grad_params, void* stream);
+
+/*
  * Fused UV texture sampling (additional entry points, no counterpart in pytorch3d._C): what
  * pytorch3d/renderer/mesh/textures.py TexturesUV.sample_textures computes for a texture with one map per mesh -- the
  * slot's UV interpolated from its face's corner UVs ((0, 0) where pix_to_face < 0), mapped to grid coordinates with

@@ -711,6 +711,111 @@ def shading_backward(grad_colors: torch.Tensor, grad_positions, pix_to_face: tor
     return g_tx, g_bary, g_fp, g_fn, g_prm
 
 
+def _check_gouraud_inputs(verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params, faces, pix_to_face,
+                          barycentric_coords, light):
+    """The device; raises RuntimeError naming the argument for anything the kernels cannot take."""
+    if light not in LIGHT_KINDS:
+        raise RuntimeError("light must be one of %s, got %r" % (sorted(LIGHT_KINDS), light))
+    if light != "ambient" and normals is None:
+        raise RuntimeError("normals are required for %s light" % light)
+    floats = [("verts", verts), ("verts_colors", verts_colors), ("params", params),
+              ("barycentric_coords", barycentric_coords)]
+    if normals is not None:
+        floats.append(("normals", normals))
+    dev = _check_blend_inputs(floats, pix_to_face)
+    _require_cuda(("faces", faces), ("mesh_first_vert", mesh_first_vert), ("mesh_num_verts", mesh_num_verts),
+                  ("pix_to_face", pix_to_face))
+    V = int(verts.shape[0]) if verts.dim() == 2 else -1
+    for name, t in floats:
+        if name in ("verts", "verts_colors", "normals") and (t.dim() != 2 or tuple(t.shape) != (V, 3)):
+            raise RuntimeError("%s must be (V, 3) with the V of verts, got %s" % (name, tuple(t.shape)))
+    for name, t in (("faces", faces), ("mesh_first_vert", mesh_first_vert), ("mesh_num_verts", mesh_num_verts)):
+        if t.dtype != torch.int64:
+            raise RuntimeError("expected scalar type Long but found %s for %s" % (t.dtype, name))
+    if faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError("faces must be (F, 3), got %s" % (tuple(faces.shape),))
+    meshes = int(mesh_first_vert.shape[0]) if mesh_first_vert.dim() == 1 else -1
+    if meshes < 0 or tuple(mesh_num_verts.shape) != (meshes,):
+        raise RuntimeError("mesh_first_vert and mesh_num_verts must be (meshes,), got %s and %s"
+                           % (tuple(mesh_first_vert.shape), tuple(mesh_num_verts.shape)))
+    if meshes > 65535:
+        raise RuntimeError("at most 65535 meshes per call, got %d" % meshes)
+    if tuple(params.shape) != (meshes, SHADING_PARAMS):
+        raise RuntimeError("params must be (meshes, %d), got %s" % (SHADING_PARAMS, tuple(params.shape)))
+    if tuple(barycentric_coords.shape) != tuple(pix_to_face.shape) + (3,):
+        raise RuntimeError("barycentric_coords must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
+                           % (tuple(barycentric_coords.shape),))
+    return dev
+
+
+def gouraud_forward(verts: torch.Tensor, normals, verts_colors: torch.Tensor, mesh_first_vert: torch.Tensor,
+                    mesh_num_verts: torch.Tensor, params: torch.Tensor, faces: torch.Tensor, pix_to_face: torch.Tensor,
+                    barycentric_coords: torch.Tensor, light: str):
+    """Fused Gouraud shading (no counterpart in pytorch3d._C; DESIGN.md section 16): verts, normals (None for ambient
+    light), verts_colors (V,3) f32 packed; mesh_first_vert, mesh_num_verts (meshes,) i64; params (meshes,22) f32, one
+    row per mesh; faces (F,3) i64 packed; pix_to_face (N,H,W,K) i64; barycentric_coords (N,H,W,K,3) f32; light
+    "point", "directional" or "ambient".  -> (colors (N,H,W,K,3), verts_shaded (V,3))."""
+    dev = _check_gouraud_inputs(verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params, faces,
+                                pix_to_face, barycentric_coords, light)
+    lib = _lib.load()
+    V, F, meshes = int(verts.shape[0]), int(faces.shape[0]), int(mesh_first_vert.shape[0])
+    P = pix_to_face.numel()
+    v, vc, prm, fc = verts.contiguous(), verts_colors.contiguous(), params.contiguous(), faces.contiguous()
+    nrm = None if light == "ambient" else normals.contiguous()
+    first, num = mesh_first_vert.contiguous(), mesh_num_verts.contiguous()
+    p2f, bary = pix_to_face.contiguous(), barycentric_coords.contiguous()
+    with torch.cuda.device(dev):
+        shaded = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        colors = torch.empty(tuple(pix_to_face.shape) + (3,), dtype=torch.float32, device=dev)
+        _lib.check(lib.b200r_gouraud_forward(_ptr(v), _ptr(nrm), _ptr(vc), V, _ptr(first), _ptr(num), meshes,
+                                             _ptr(prm), _ptr(fc), F, _ptr(p2f), _ptr(bary), P, LIGHT_KINDS[light],
+                                             _ptr(shaded), _ptr(colors), _stream_ptr(dev)))
+    return colors, shaded
+
+
+def gouraud_backward(grad_colors: torch.Tensor, verts: torch.Tensor, normals, verts_colors: torch.Tensor,
+                     mesh_first_vert: torch.Tensor, mesh_num_verts: torch.Tensor, params: torch.Tensor,
+                     faces: torch.Tensor, pix_to_face: torch.Tensor, barycentric_coords: torch.Tensor, light: str,
+                     verts_shaded: torch.Tensor, needs_input_grad=(True, True, True, True, True)):
+    """Backward of `gouraud_forward` -> (grad_verts, grad_normals, grad_verts_colors, grad_barycentric_coords,
+    grad_params); an entry is None where `needs_input_grad` (same order) is false.  grad_barycentric_coords is
+    deterministic; the other four start from a per-vertex sum accumulated with atomics, so requesting them under
+    torch.use_deterministic_algorithms(True) raises, as the reference's interpolation backward does."""
+    dev = _check_gouraud_inputs(verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params, faces,
+                                pix_to_face, barycentric_coords, light)
+    _require_cuda(("grad_colors", grad_colors), ("verts_shaded", verts_shaded), ("pix_to_face", pix_to_face))
+    if grad_colors.dtype != torch.float32 or tuple(grad_colors.shape) != tuple(pix_to_face.shape) + (3,):
+        raise RuntimeError("grad_colors must be a float32 tensor of shape (N, H, W, K, 3)")
+    if verts_shaded.dtype != torch.float32 or tuple(verts_shaded.shape) != tuple(verts.shape):
+        raise RuntimeError("verts_shaded must be a float32 tensor of shape (V, 3)")
+    need_v, need_n, need_vc, need_bary, need_prm = (bool(x) for x in needs_input_grad)
+    need_n = need_n and normals is not None
+    if ((need_v or need_n or need_vc or need_prm) and torch.are_deterministic_algorithms_enabled()
+            and not torch.is_deterministic_algorithms_warn_only_enabled()):
+        raise RuntimeError(
+            "gouraud_backward does not have a deterministic implementation (the gradient of the shaded vertex colours "
+            "is accumulated with atomics), but you set 'torch.use_deterministic_algorithms(True)'.")
+    lib = _lib.load()
+    V, F, meshes = int(verts.shape[0]), int(faces.shape[0]), int(mesh_first_vert.shape[0])
+    P = pix_to_face.numel()
+    gc, v, vc, prm = grad_colors.contiguous(), verts.contiguous(), verts_colors.contiguous(), params.contiguous()
+    nrm = None if light == "ambient" else normals.contiguous()
+    first, num, fc = mesh_first_vert.contiguous(), mesh_num_verts.contiguous(), faces.contiguous()
+    p2f, bary, shaded = pix_to_face.contiguous(), barycentric_coords.contiguous(), verts_shaded.contiguous()
+    with torch.cuda.device(dev):
+        def out(flag, shape):
+            return torch.empty(shape, dtype=torch.float32, device=dev) if flag else None
+        g_v, g_n, g_vc = out(need_v, (V, 3)), out(need_n, (V, 3)), out(need_vc, (V, 3))
+        g_bary, g_prm = out(need_bary, tuple(barycentric_coords.shape)), out(need_prm, (meshes, SHADING_PARAMS))
+        ws_bytes = int(lib.b200r_gouraud_workspace_bytes(meshes, V)) if (need_v or need_n or need_vc or need_prm) else 0
+        ws = torch.empty((ws_bytes // 4,), dtype=torch.float32, device=dev) if ws_bytes else None
+        _lib.check(lib.b200r_gouraud_backward(
+            _ptr(gc), _ptr(v), _ptr(nrm), _ptr(vc), V, _ptr(first), _ptr(num), meshes, _ptr(prm), _ptr(fc), F,
+            _ptr(p2f), _ptr(bary), P, LIGHT_KINDS[light], _ptr(shaded), _ptr(ws), ws_bytes, _ptr(g_v), _ptr(g_n),
+            _ptr(g_vc), _ptr(g_bary), _ptr(g_prm), _stream_ptr(dev)))
+    return g_v, g_n, g_vc, g_bary, g_prm
+
+
 SAMPLING_MODES = {"bilinear": 0, "nearest": 1}  # B200R_SAMPLE_*: torch's GridSamplerInterpolation
 PADDING_MODES = {"zeros": 0, "border": 1, "reflection": 2}  # B200R_PAD_*: torch's GridSamplerPadding
 

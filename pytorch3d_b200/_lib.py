@@ -80,6 +80,13 @@ SIGNATURES = {
         ctypes.c_int,
         [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp, _vp, _vp,
          _vp, _vp, _vp]),
+    "b200r_gouraud_forward": (
+        ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp]),
+    "b200r_gouraud_workspace_bytes": (_sz, [_i32, _i64]),
+    "b200r_gouraud_backward": (
+        ctypes.c_int,
+        [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _sz, _vp, _vp, _vp,
+         _vp, _vp, _vp]),
     "b200r_texture_uv_forward": (
         ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "b200r_texture_uv_backward": (

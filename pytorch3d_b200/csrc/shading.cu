@@ -1,4 +1,4 @@
-// Phong and flat shading, forward and backward (DESIGN.md section 12).
+// Phong and flat shading, forward and backward (DESIGN.md section 12), and Gouraud shading (section 16, below).
 //
 // What pytorch3d/renderer/mesh/shading.py (_phong_shading_with_pixels, phong_shading, flat_shading) computes with the
 // light models of renderer/lighting.py (PointLights, DirectionalLights, AmbientLights), per rasterized slot:
@@ -163,15 +163,72 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 
-// Adds one warp's per-slot face gradients into `out` (M floats per face).  All lanes that hold the same face are merged
-// first (one MATCH, then pointer jumping as in the rasterizer's backward, DESIGN.md section 6), so every distinct face of
-// the warp costs one set of M atomics.  Every lane of the warp must call it; lanes without a face pass face = -1.
+// Gradient of one point's colour (ambient + diffuse) * texel + specular (light_slot, compose) for the upstream g: the
+// texel gradient goes to row i of gtex (i * 3 + c; gtex may be null), the position and normal gradients are added into gp and gn
+// (left as they are for ambient light), and with PARAMS every parameter gradient is added into acc.
+template <int LIGHT, bool PARAMS>
+__device__ __forceinline__ void lighting_backward(const float* prm, const Lit& t, V3 n, V3 g, V3 tx, float* gtex,
+                                                  int64_t i, V3& gp, V3& gn, float (&acc)[kP]) {
+  const float gc[3] = {g.x, g.y, g.z}, tc[3] = {tx.x, tx.y, tx.z};
+  float g_angle = 0.0f, g_pw = 0.0f;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float md = __ldg(prm + MD + c), ld = __ldg(prm + LD + c);
+    const float ms = __ldg(prm + MS + c), ls = __ldg(prm + LS + c);
+    const float ldang = fmul(ld, t.angle), lspow = fmul(ls, t.pw);
+    if (gtex != nullptr) gtex[i * 3 + c] = fmul(gc[c], fadd(__ldg(prm + AMB + c), fmul(md, ldang)));
+    const float gd = gc[c] * tc[c];  // gradient of the diffuse colour
+    const float g_ldang = gd * md, g_lspow = gc[c] * ms;
+    if (PARAMS) {
+      acc[AMB + c] += gd;
+      acc[MD + c] += gd * ldang;
+      acc[LD + c] += g_ldang * t.angle;
+      acc[MS + c] += gc[c] * lspow;
+      acc[LS + c] += g_lspow * t.pw;
+    }
+    g_angle += g_ldang * ld;
+    g_pw += g_lspow * ls;
+  }
+  if (LIGHT != B200R_LIGHT_AMBIENT) {
+    // pow: no gradient to the base where the exponent is 0, none to the exponent where the base is 0 (exponent >= 0)
+    const float g_alpha = t.shin == 0.0f ? 0.0f : g_pw * (t.shin * powf(t.alpha, t.shin - 1.0f));
+    if (PARAMS && !(t.alpha == 0.0f && t.shin >= 0.0f)) acc[SHIN] += g_pw * (t.pw * logf(t.alpha));
+    // alpha = relu(<vn, R>) * (cos > 0): relu and the mask pass nothing at 0
+    const float g_dot = (t.cos > 0.0f && t.dot_vr > 0.0f) ? g_alpha : 0.0f;
+    const V3 g_vn = {g_dot * t.R.x, g_dot * t.R.y, g_dot * t.R.z};
+    const V3 g_R = {g_dot * t.vn.u.x, g_dot * t.vn.u.y, g_dot * t.vn.u.z};
+    // R = -ln + 2 * (cos * nn); angle = relu(cos); cos = <nn, ln>
+    const float g_cos = 2.0f * dot3(g_R, t.nn.u) + (t.angle > 0.0f ? g_angle : 0.0f);
+    const V3 g_nn = {2.0f * g_R.x * t.cos + g_cos * t.ln.u.x, 2.0f * g_R.y * t.cos + g_cos * t.ln.u.y,
+                     2.0f * g_R.z * t.cos + g_cos * t.ln.u.z};
+    const V3 g_ln = {g_cos * t.nn.u.x - g_R.x, g_cos * t.nn.u.y - g_R.y, g_cos * t.nn.u.z - g_R.z};
+    gn = normalize3_backward(n, t.nn, g_nn);
+    const V3 g_L = normalize3_backward(t.L, t.ln, g_ln);
+    const V3 g_V = normalize3_backward(t.V, t.vn, g_vn);
+    gp = {-g_V.x, -g_V.y, -g_V.z};
+    if (LIGHT == B200R_LIGHT_POINT) {
+      gp = {gp.x - g_L.x, gp.y - g_L.y, gp.z - g_L.z};
+    }
+    if (PARAMS) {
+      acc[LOC + 0] += g_L.x;
+      acc[LOC + 1] += g_L.y;
+      acc[LOC + 2] += g_L.z;
+      acc[CAM + 0] += g_V.x;
+      acc[CAM + 1] += g_V.y;
+      acc[CAM + 2] += g_V.z;
+    }
+  }
+}
+
+// Merges one warp's per-lane gradients (M floats each) over the lanes that hold the same key: one MATCH, then pointer
+// jumping as in the rasterizer's backward (DESIGN.md section 6).  Returns true on the one lane per distinct key >= 0
+// that holds its key's sum.  Every lane of the warp must call it; lanes without a key pass key = -1.
 template <int M>
-__device__ __forceinline__ void warp_scatter(float* __restrict__ out, int64_t face, float (&g)[M]) {
+__device__ __forceinline__ bool warp_merge(int64_t key, float (&g)[M]) {
   const int lane = threadIdx.x & 31;
-  const unsigned grp = __match_any_sync(0xffffffffu, face);
+  const unsigned grp = __match_any_sync(0xffffffffu, key);
   const unsigned above = lane == 31 ? 0u : grp & (0xffffffffu << (lane + 1));
-  int next = (face >= 0 && above != 0u) ? __ffs((int)above) - 1 : -1;
+  int next = (key >= 0 && above != 0u) ? __ffs((int)above) - 1 : -1;
   while (__any_sync(0xffffffffu, next >= 0)) {
     const int src = next >= 0 ? next : lane;
 #pragma unroll
@@ -182,7 +239,14 @@ __device__ __forceinline__ void warp_scatter(float* __restrict__ out, int64_t fa
     const int nn = __shfl_sync(0xffffffffu, next, src);
     next = next >= 0 ? nn : -1;
   }
-  if (face >= 0 && lane == __ffs((int)grp) - 1) {
+  return key >= 0 && lane == __ffs((int)grp) - 1;
+}
+
+// Adds one warp's per-slot face gradients into `out` (M floats per face), so every distinct face of the warp costs one
+// set of M atomics.  Every lane of the warp must call it; lanes without a face pass face = -1.
+template <int M>
+__device__ __forceinline__ void warp_scatter(float* __restrict__ out, int64_t face, float (&g)[M]) {
+  if (warp_merge<M>(face, g)) {
     float* o = out + face * M;
 #pragma unroll
     for (int i = 0; i < M; ++i) atomicAdd(o + i, g[i]);
@@ -205,6 +269,26 @@ struct BackwardArgs {
   float* grad_face_nrm;  // may be null
   float* partials;       // (N, gridDim.x, kP) when PARAMS
 };
+
+// The CTA's sum of every thread's acc, written to row[0:kP]: a fixed-order reduction, butterfly within warps, then
+// warps 0..7 in order.  Every thread of the CTA must call it.
+__device__ __forceinline__ void store_partial_row(const float (&acc)[kP], float* row) {
+  __shared__ float red[kThreads / 32][kP];
+#pragma unroll
+  for (int i = 0; i < kP; ++i) {
+    float v = acc[i];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5][i] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < kP) {
+    float v = 0.0f;
+#pragma unroll
+    for (int wi = 0; wi < kThreads / 32; ++wi) v += red[wi][threadIdx.x];
+    row[threadIdx.x] = v;
+  }
+}
 
 // grid (blocks per image, N): a CTA only sees the slots of one image, so its parameter gradients are one partial row.
 template <bool FLAT, int LIGHT, bool PARAMS>
@@ -229,57 +313,8 @@ __global__ void __launch_bounds__(kThreads) shading_backward_kernel(const Backwa
     if (active) {
       Lit t;
       light_slot<LIGHT>(p, n, prm, t);
-      const V3 g = ld3(a.grad_colors + s * 3), tx = ld3(a.texels + s * 3);
-      const float gc[3] = {g.x, g.y, g.z}, tc[3] = {tx.x, tx.y, tx.z};
-      float g_angle = 0.0f, g_pw = 0.0f;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const float md = __ldg(prm + MD + c), ld = __ldg(prm + LD + c);
-        const float ms = __ldg(prm + MS + c), ls = __ldg(prm + LS + c);
-        const float ldang = fmul(ld, t.angle), lspow = fmul(ls, t.pw);
-        if (a.grad_texels != nullptr)
-          a.grad_texels[s * 3 + c] = fmul(gc[c], fadd(__ldg(prm + AMB + c), fmul(md, ldang)));
-        const float gd = gc[c] * tc[c];  // gradient of the diffuse colour
-        const float g_ldang = gd * md, g_lspow = gc[c] * ms;
-        if (PARAMS) {
-          acc[AMB + c] += gd;
-          acc[MD + c] += gd * ldang;
-          acc[LD + c] += g_ldang * t.angle;
-          acc[MS + c] += gc[c] * lspow;
-          acc[LS + c] += g_lspow * t.pw;
-        }
-        g_angle += g_ldang * ld;
-        g_pw += g_lspow * ls;
-      }
-      if (LIGHT != B200R_LIGHT_AMBIENT) {
-        // pow: no gradient to the base where the exponent is 0, none to the exponent where the base is 0 (exponent >= 0)
-        const float g_alpha = t.shin == 0.0f ? 0.0f : g_pw * (t.shin * powf(t.alpha, t.shin - 1.0f));
-        if (PARAMS && !(t.alpha == 0.0f && t.shin >= 0.0f)) acc[SHIN] += g_pw * (t.pw * logf(t.alpha));
-        // alpha = relu(<vn, R>) * (cos > 0): relu and the mask pass nothing at 0
-        const float g_dot = (t.cos > 0.0f && t.dot_vr > 0.0f) ? g_alpha : 0.0f;
-        const V3 g_vn = {g_dot * t.R.x, g_dot * t.R.y, g_dot * t.R.z};
-        const V3 g_R = {g_dot * t.vn.u.x, g_dot * t.vn.u.y, g_dot * t.vn.u.z};
-        // R = -ln + 2 * (cos * nn); angle = relu(cos); cos = <nn, ln>
-        const float g_cos = 2.0f * dot3(g_R, t.nn.u) + (t.angle > 0.0f ? g_angle : 0.0f);
-        const V3 g_nn = {2.0f * g_R.x * t.cos + g_cos * t.ln.u.x, 2.0f * g_R.y * t.cos + g_cos * t.ln.u.y,
-                         2.0f * g_R.z * t.cos + g_cos * t.ln.u.z};
-        const V3 g_ln = {g_cos * t.nn.u.x - g_R.x, g_cos * t.nn.u.y - g_R.y, g_cos * t.nn.u.z - g_R.z};
-        gn = normalize3_backward(n, t.nn, g_nn);
-        const V3 g_L = normalize3_backward(t.L, t.ln, g_ln);
-        const V3 g_V = normalize3_backward(t.V, t.vn, g_vn);
-        gp = {-g_V.x, -g_V.y, -g_V.z};
-        if (LIGHT == B200R_LIGHT_POINT) {
-          gp = {gp.x - g_L.x, gp.y - g_L.y, gp.z - g_L.z};
-        }
-        if (PARAMS) {
-          acc[LOC + 0] += g_L.x;
-          acc[LOC + 1] += g_L.y;
-          acc[LOC + 2] += g_L.z;
-          acc[CAM + 0] += g_V.x;
-          acc[CAM + 1] += g_V.y;
-          acc[CAM + 2] += g_V.z;
-        }
-      }
+      lighting_backward<LIGHT, PARAMS>(prm, t, n, ld3(a.grad_colors + s * 3), ld3(a.texels + s * 3),
+                                       a.grad_texels, s, gp, gn, acc);
       if (a.grad_positions != nullptr) {
         const V3 u = ld3(a.grad_positions + s * 3);
         gp = {gp.x + u.x, gp.y + u.y, gp.z + u.z};
@@ -320,23 +355,7 @@ __global__ void __launch_bounds__(kThreads) shading_backward_kernel(const Backwa
       warp_scatter<3 * CORNERS>(a.grad_face_nrm, f, g);
     }
   }
-  if (PARAMS) {  // fixed-order CTA reduction: butterfly within warps, then warps 0..7 in order
-    __shared__ float red[kThreads / 32][kP];
-#pragma unroll
-    for (int i = 0; i < kP; ++i) {
-      float v = acc[i];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5][i] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < kP) {
-      float v = 0.0f;
-#pragma unroll
-      for (int wi = 0; wi < kThreads / 32; ++wi) v += red[wi][threadIdx.x];
-      a.partials[(img * gridDim.x + blockIdx.x) * kP + threadIdx.x] = v;
-    }
-  }
+  if (PARAMS) store_partial_row(acc, a.partials + (img * gridDim.x + blockIdx.x) * kP);
 }
 
 // grad_params[n, j] = sum over the CTAs b of image n, in order, of partials[n, b, j]
@@ -393,6 +412,186 @@ void launch_backward_mode(bool flat, const BackwardArgs& a, dim3 grid, bool para
     launch_backward<true, LIGHT>(a, grid, params, stream);
   else
     launch_backward<false, LIGHT>(a, grid, params, stream);
+}
+
+// ---- Gouraud shading (DESIGN.md section 16) ----
+// The vertex stage lights every vertex with its mesh's parameter row (light_slot, compose); the slot stage interpolates
+// the shaded vertex colours with interp_face_attrs_forward_kernel's FMA chain.  Vertex-stage grids are
+// (blocks per mesh, meshes); a CTA strides over its mesh's vertex range [first[m], first[m] + num[m]).
+
+template <int LIGHT>
+__global__ void __launch_bounds__(kThreads)
+    gouraud_vertex_forward_kernel(const float* __restrict__ verts, const float* __restrict__ normals,
+                                  const float* __restrict__ verts_colors, const int64_t* __restrict__ first,
+                                  const int64_t* __restrict__ num, const float* __restrict__ params,
+                                  float* __restrict__ verts_shaded) {
+  const int64_t m = blockIdx.y;
+  const float* prm = params + m * kP;
+  const int64_t v0 = __ldg(first + m), v1 = v0 + __ldg(num + m);
+  for (int64_t v = v0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < v1; v += (int64_t)gridDim.x * blockDim.x) {
+    V3 p = {0.0f, 0.0f, 0.0f}, n = {0.0f, 0.0f, 0.0f};
+    if (LIGHT != B200R_LIGHT_AMBIENT) {
+      p = ld3(verts + v * 3);
+      n = ld3(normals + v * 3);
+    }
+    Lit t;
+    light_slot<LIGHT>(p, n, prm, t);
+    const V3 c = ld3(verts_colors + v * 3);
+    verts_shaded[v * 3 + 0] = compose(prm, 0, t.angle, t.pw, c.x);
+    verts_shaded[v * 3 + 1] = compose(prm, 1, t.angle, t.pw, c.y);
+    verts_shaded[v * 3 + 2] = compose(prm, 2, t.angle, t.pw, c.z);
+  }
+}
+
+__global__ void __launch_bounds__(kThreads)
+    gouraud_slot_forward_kernel(const int64_t* __restrict__ pix_to_face, const float* __restrict__ bary,
+                                const int64_t* __restrict__ faces, const float* __restrict__ verts_shaded, int64_t P,
+                                float* __restrict__ colors) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < P; s += stride) {
+    const int64_t f = __ldg(pix_to_face + s);
+    float c[3] = {0.0f, 0.0f, 0.0f};
+    if (f >= 0) {
+      const float w0 = __ldg(bary + s * 3 + 0), w1 = __ldg(bary + s * 3 + 1), w2 = __ldg(bary + s * 3 + 2);
+      const float* a0 = verts_shaded + __ldg(faces + f * 3 + 0) * 3;
+      const float* a1 = verts_shaded + __ldg(faces + f * 3 + 1) * 3;
+      const float* a2 = verts_shaded + __ldg(faces + f * 3 + 2) * 3;
+#pragma unroll
+      for (int d = 0; d < 3; ++d) c[d] = ffma(w2, __ldg(a2 + d), ffma(w1, __ldg(a1 + d), ffma(w0, __ldg(a0 + d), 0.0f)));
+    }
+    colors[s * 3 + 0] = c[0];
+    colors[s * 3 + 1] = c[1];
+    colors[s * 3 + 2] = c[2];
+  }
+}
+
+// grad_bary[s, i] = <verts_shaded[v_i], g> as interp_face_attrs_backward_kernel rounds it (one FMA per channel, from
+// 0); w_i * g is merged over the warp's lanes of the same face, then added to the face's three rows of grad_shaded.
+__global__ void __launch_bounds__(kThreads)
+    gouraud_slot_backward_kernel(const float* __restrict__ grad_colors, const int64_t* __restrict__ pix_to_face,
+                                 const float* __restrict__ bary, const int64_t* __restrict__ faces,
+                                 const float* __restrict__ verts_shaded, int64_t P, float* __restrict__ grad_bary,
+                                 float* __restrict__ grad_shaded) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  // warp-uniform trip count: every lane reaches the warp-wide merge
+  for (int64_t s0 = (int64_t)blockIdx.x * blockDim.x; s0 < P; s0 += stride) {
+    const int64_t s = s0 + threadIdx.x;
+    const bool active = s < P;
+    const int64_t f = active ? __ldg(pix_to_face + s) : -1;
+    float g[9] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+    int64_t vi[3] = {0, 0, 0};
+    if (f >= 0) {
+      const V3 u = ld3(grad_colors + s * 3);
+      const float w[3] = {__ldg(bary + s * 3 + 0), __ldg(bary + s * 3 + 1), __ldg(bary + s * 3 + 2)};
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        vi[i] = __ldg(faces + f * 3 + i);
+        g[3 * i + 0] = w[i] * u.x;
+        g[3 * i + 1] = w[i] * u.y;
+        g[3 * i + 2] = w[i] * u.z;
+      }
+      if (grad_bary != nullptr) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+          const V3 a = ld3(verts_shaded + vi[i] * 3);
+          grad_bary[s * 3 + i] = ffma(a.z, u.z, ffma(a.y, u.y, ffma(a.x, u.x, 0.0f)));
+        }
+      }
+    } else if (active && grad_bary != nullptr) {
+      grad_bary[s * 3 + 0] = 0.0f;
+      grad_bary[s * 3 + 1] = 0.0f;
+      grad_bary[s * 3 + 2] = 0.0f;
+    }
+    if (grad_shaded != nullptr && warp_merge<9>(f, g)) {
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        float* o = grad_shaded + vi[i] * 3;
+        atomicAdd(o + 0, g[3 * i + 0]);
+        atomicAdd(o + 1, g[3 * i + 1]);
+        atomicAdd(o + 2, g[3 * i + 2]);
+      }
+    }
+  }
+}
+
+struct GouraudBackwardArgs {
+  const float* grad_shaded;
+  const float* verts;
+  const float* normals;
+  const float* verts_colors;
+  const int64_t* first;
+  const int64_t* num;
+  const float* params;
+  float* grad_verts;         // may be null
+  float* grad_normals;       // may be null
+  float* grad_verts_colors;  // may be null
+  float* partials;           // (meshes, gridDim.x, kP) when PARAMS
+};
+
+// Same grid as the vertex forward; every vertex's gradients are written once, the parameter gradients go to one
+// partial row per CTA.
+template <int LIGHT, bool PARAMS>
+__global__ void __launch_bounds__(kThreads) gouraud_vertex_backward_kernel(const GouraudBackwardArgs a) {
+  const int64_t m = blockIdx.y;
+  const float* prm = a.params + m * kP;
+  float acc[kP];
+#pragma unroll
+  for (int i = 0; i < kP; ++i) acc[i] = 0.0f;
+  const int64_t v0 = __ldg(a.first + m), v1 = v0 + __ldg(a.num + m);
+  for (int64_t v = v0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < v1; v += (int64_t)gridDim.x * blockDim.x) {
+    V3 p = {0.0f, 0.0f, 0.0f}, n = {0.0f, 0.0f, 0.0f};
+    if (LIGHT != B200R_LIGHT_AMBIENT) {
+      p = ld3(a.verts + v * 3);
+      n = ld3(a.normals + v * 3);
+    }
+    Lit t;
+    light_slot<LIGHT>(p, n, prm, t);
+    V3 gp = {0.0f, 0.0f, 0.0f}, gn = {0.0f, 0.0f, 0.0f};
+    lighting_backward<LIGHT, PARAMS>(prm, t, n, ld3(a.grad_shaded + v * 3), ld3(a.verts_colors + v * 3),
+                                     a.grad_verts_colors, v, gp, gn, acc);
+    if (a.grad_verts != nullptr) {
+      a.grad_verts[v * 3 + 0] = gp.x;
+      a.grad_verts[v * 3 + 1] = gp.y;
+      a.grad_verts[v * 3 + 2] = gp.z;
+    }
+    if (a.grad_normals != nullptr) {
+      a.grad_normals[v * 3 + 0] = gn.x;
+      a.grad_normals[v * 3 + 1] = gn.y;
+      a.grad_normals[v * 3 + 2] = gn.z;
+    }
+  }
+  if (PARAMS) store_partial_row(acc, a.partials + (m * gridDim.x + blockIdx.x) * kP);
+}
+
+// CTAs per mesh of the vertex stage: enough for the mean mesh size, capped like the slot backward's.  A function of
+// (V, meshes) only, so that the parameter gradients are summed in the same order on every GPU.
+int gouraud_blocks_per_mesh(int32_t meshes, int64_t V) {
+  if (meshes <= 0) return 1;
+  const int64_t want = (V + (int64_t)meshes * kThreads - 1) / ((int64_t)meshes * kThreads);
+  const int64_t cap = (int64_t)4224 / meshes;
+  int64_t b = want < cap ? want : cap;
+  return (int)(b < 1 ? 1 : b);
+}
+
+size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
+
+template <int LIGHT>
+void launch_gouraud_vertex_backward(const GouraudBackwardArgs& a, dim3 grid, bool params, cudaStream_t stream) {
+  if (params)
+    gouraud_vertex_backward_kernel<LIGHT, true><<<grid, kThreads, 0, stream>>>(a);
+  else
+    gouraud_vertex_backward_kernel<LIGHT, false><<<grid, kThreads, 0, stream>>>(a);
+}
+
+int check_gouraud_args(int64_t V, int32_t meshes, int64_t F, int64_t P, int32_t light, const float* normals) {
+  if (V < 0 || meshes < 0 || F < 0 || P < 0) return fail(B200R_ERR_INVALID_ARGUMENT, "negative size");
+  if (light != B200R_LIGHT_POINT && light != B200R_LIGHT_DIRECTIONAL && light != B200R_LIGHT_AMBIENT)
+    return fail(B200R_ERR_INVALID_ARGUMENT, "unknown light kind");
+  if (light != B200R_LIGHT_AMBIENT && normals == nullptr && V > 0)
+    return fail(B200R_ERR_INVALID_ARGUMENT, "gouraud shading needs vertex normals for a point or directional light");
+  if (meshes > 65535) return fail(B200R_ERR_INVALID_ARGUMENT, "gouraud shading: at most 65535 meshes per call");
+  if (meshes == 0 && V > 0) return fail(B200R_ERR_INVALID_ARGUMENT, "gouraud shading: vertices but no meshes");
+  return B200R_OK;
 }
 
 int check_shading_args(int32_t N, int32_t H, int32_t W, int32_t K, int64_t F, int32_t flat, int32_t light,
@@ -482,6 +681,99 @@ extern "C" int b200r_shading_backward(const float* grad_colors, const float* gra
     const int64_t n = (int64_t)N * kP;
     shading_params_sum_kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, stream>>>(
         static_cast<const float*>(workspace), bpi, N, grad_params);
+    B200R_LAUNCHED("shading_params_sum_kernel");
+  }
+  return B200R_OK;
+}
+
+extern "C" int b200r_gouraud_forward(const float* verts, const float* normals, const float* verts_colors, int64_t V,
+                                     const int64_t* mesh_first_vert, const int64_t* mesh_num_verts, int32_t meshes,
+                                     const float* params, const int64_t* faces, int64_t F, const int64_t* pix_to_face,
+                                     const float* barycentric_coords, int64_t P, int32_t light, float* verts_shaded,
+                                     float* colors, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int rc = check_gouraud_args(V, meshes, F, P, light, normals);
+  if (rc != B200R_OK) return rc;
+  if (V > 0 && meshes > 0) {
+    const dim3 grid((unsigned)gouraud_blocks_per_mesh(meshes, V), (unsigned)meshes);
+    if (light == B200R_LIGHT_POINT)
+      gouraud_vertex_forward_kernel<B200R_LIGHT_POINT><<<grid, kThreads, 0, stream>>>(
+          verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params, verts_shaded);
+    else if (light == B200R_LIGHT_DIRECTIONAL)
+      gouraud_vertex_forward_kernel<B200R_LIGHT_DIRECTIONAL><<<grid, kThreads, 0, stream>>>(
+          verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params, verts_shaded);
+    else
+      gouraud_vertex_forward_kernel<B200R_LIGHT_AMBIENT><<<grid, kThreads, 0, stream>>>(
+          verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params, verts_shaded);
+    B200R_LAUNCHED("gouraud_vertex_forward_kernel");
+  }
+  if (P > 0) {
+    const int64_t blocks = cap_grid_stride_blocks((P + kThreads - 1) / kThreads);
+    gouraud_slot_forward_kernel<<<(unsigned)blocks, kThreads, 0, stream>>>(pix_to_face, barycentric_coords, faces,
+                                                                          verts_shaded, P, colors);
+    B200R_LAUNCHED("gouraud_slot_forward_kernel");
+  }
+  return B200R_OK;
+}
+
+extern "C" size_t b200r_gouraud_workspace_bytes(int32_t meshes, int64_t V) {
+  if (meshes < 0 || V < 0) return 0;
+  return align256(sizeof(float) * (size_t)V * 3) +
+         sizeof(float) * (size_t)meshes * (size_t)gouraud_blocks_per_mesh(meshes, V) * kP;
+}
+
+extern "C" int b200r_gouraud_backward(const float* grad_colors, const float* verts, const float* normals,
+                                      const float* verts_colors, int64_t V, const int64_t* mesh_first_vert,
+                                      const int64_t* mesh_num_verts, int32_t meshes, const float* params,
+                                      const int64_t* faces, int64_t F, const int64_t* pix_to_face,
+                                      const float* barycentric_coords, int64_t P, int32_t light,
+                                      const float* verts_shaded, void* workspace, size_t workspace_bytes,
+                                      float* grad_verts, float* grad_normals, float* grad_verts_colors,
+                                      float* grad_barycentric_coords, float* grad_params, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int rc = check_gouraud_args(V, meshes, F, P, light, normals);
+  if (rc != B200R_OK) return rc;
+  const bool want_vertex = grad_verts != nullptr || grad_normals != nullptr || grad_verts_colors != nullptr ||
+                           grad_params != nullptr;
+  if (want_vertex && (workspace == nullptr || workspace_bytes < b200r_gouraud_workspace_bytes(meshes, V)))
+    return fail(B200R_ERR_INVALID_ARGUMENT, "gouraud backward: workspace too small");
+  float* grad_shaded = want_vertex ? static_cast<float*>(workspace) : nullptr;
+  float* partials = want_vertex ? reinterpret_cast<float*>(static_cast<char*>(workspace) +
+                                                           align256(sizeof(float) * (size_t)V * 3))
+                                : nullptr;
+  if (grad_shaded != nullptr && V > 0)
+    B200R_CUDA_OK(cudaMemsetAsync(grad_shaded, 0, sizeof(float) * (size_t)V * 3, stream));
+  if (P > 0 && (grad_shaded != nullptr || grad_barycentric_coords != nullptr)) {
+    const int64_t blocks = cap_grid_stride_blocks((P + kThreads - 1) / kThreads);
+    gouraud_slot_backward_kernel<<<(unsigned)blocks, kThreads, 0, stream>>>(
+        grad_colors, pix_to_face, barycentric_coords, faces, verts_shaded, P, grad_barycentric_coords, grad_shaded);
+    B200R_LAUNCHED("gouraud_slot_backward_kernel");
+  }
+  if (!want_vertex || meshes == 0) return B200R_OK;
+  if (V == 0) {
+    if (grad_params != nullptr)
+      B200R_CUDA_OK(cudaMemsetAsync(grad_params, 0, sizeof(float) * (size_t)meshes * kP, stream));
+    return B200R_OK;
+  }
+  const int bpm = gouraud_blocks_per_mesh(meshes, V);
+  const GouraudBackwardArgs a{grad_shaded, verts,      normals,           verts_colors,
+                              mesh_first_vert, mesh_num_verts, params, grad_verts,
+                              light == B200R_LIGHT_AMBIENT ? nullptr : grad_normals, grad_verts_colors, partials};
+  const dim3 grid((unsigned)bpm, (unsigned)meshes);
+  const bool want_params = grad_params != nullptr;
+  if (light == B200R_LIGHT_POINT)
+    launch_gouraud_vertex_backward<B200R_LIGHT_POINT>(a, grid, want_params, stream);
+  else if (light == B200R_LIGHT_DIRECTIONAL)
+    launch_gouraud_vertex_backward<B200R_LIGHT_DIRECTIONAL>(a, grid, want_params, stream);
+  else
+    launch_gouraud_vertex_backward<B200R_LIGHT_AMBIENT>(a, grid, want_params, stream);
+  B200R_LAUNCHED("gouraud_vertex_backward_kernel");
+  if (light == B200R_LIGHT_AMBIENT && grad_normals != nullptr)
+    B200R_CUDA_OK(cudaMemsetAsync(grad_normals, 0, sizeof(float) * (size_t)V * 3, stream));
+  if (want_params) {
+    const int64_t n = (int64_t)meshes * kP;
+    shading_params_sum_kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, stream>>>(partials, bpm,
+                                                                                                  meshes, grad_params);
     B200R_LAUNCHED("shading_params_sum_kernel");
   }
   return B200R_OK;

@@ -34,6 +34,16 @@ It replaces the three functions in both modules by functions that send float32 C
 PointLights / DirectionalLights / AmbientLights and Materials to `pytorch3d_b200.shading`, and everything else to the
 originals.
 
+`install_gouraud()` (separate again, so that `install_shading()` keeps its three functions) serves the per-vertex
+lighting of SoftGouraudShader and HardGouraudShader:
+    pytorch3d/renderer/mesh/shading.py      gouraud_shading (pure torch: per-vertex lighting, a gather, interpolation)
+    pytorch3d/renderer/mesh/shader.py       from .shading import gouraud_shading, ...
+It replaces the function in both modules by one that sends float32 CUDA vertices, vertex colours and barycentrics
+with int64 CUDA pix_to_face, all on one device, a 3-channel `TexturesVertex`, PyTorch3D's own PointLights /
+DirectionalLights / AmbientLights and Materials, cameras with R and T, and properties and cameras of batch 1 or
+len(meshes) to `pytorch3d_b200.shading`,
+and everything else (1-channel vertex features, other textures, subclasses, CPU tensors) to the original.
+
 `install_textures()` (separate again) serves the texture sampling of every mesh shader for `TexturesUV`:
     pytorch3d/renderer/mesh/textures.py     TexturesUV.sample_textures (pure torch: interpolation, grid_sample)
 It replaces the method on the class itself, so every import path sees it.  Textures with one map per mesh (no
@@ -80,7 +90,8 @@ _TEXTURES_MODULE = "pytorch3d.renderer.mesh.textures"
 _CLIP_MODULE = "pytorch3d.renderer.mesh.rasterize_meshes"
 _CLIP_FUNCTIONS = ("clip_faces", "convert_clipped_rasterization_to_original_faces")
 _saved = {}
-# (module name, attribute) -> original (install_blending, install_splatter, install_shading and install_clipping)
+# (module name, attribute) -> original (install_blending, install_splatter, install_shading, install_gouraud and
+# install_clipping)
 _saved_blend = {}
 _saved_methods = {}  # (module name, class name, method name) -> original (install_textures, install_texture_atlas)
 
@@ -268,6 +279,72 @@ def install_shading():
     return list(_SHADING_MODULES)
 
 
+def _gouraud_fused(meshes, fragments, lights, cameras, materials):
+    """Whether the fused Gouraud shading takes this call (see the module docstring)."""
+    try:
+        lighting = importlib.import_module("pytorch3d.renderer.lighting")
+        materials_mod = importlib.import_module("pytorch3d.renderer.materials")
+        textures_mod = importlib.import_module(_TEXTURES_MODULE)
+    except ImportError:
+        return False
+    light_types = tuple(getattr(lighting, n) for n in ("PointLights", "DirectionalLights", "AmbientLights")
+                        if hasattr(lighting, n))
+    if type(lights) not in light_types or type(materials) is not getattr(materials_mod, "Materials", None):
+        return False
+    if type(getattr(meshes, "textures", None)) is not getattr(textures_mod, "TexturesVertex", None):
+        return False
+    verts, feats = meshes.verts_packed(), meshes.textures.verts_features_packed()
+    bary, p2f = getattr(fragments, "bary_coords", None), fragments.pix_to_face
+    if not all(getattr(t, "is_cuda", False) for t in (verts, feats, bary, p2f)):
+        return False
+    if verts.device != p2f.device or feats.device != p2f.device or bary.device != p2f.device:
+        return False
+    if verts.dtype != torch.float32 or feats.dtype != torch.float32 or bary.dtype != torch.float32 \
+            or p2f.dtype != torch.int64:
+        return False
+    if feats.dim() != 2 or feats.shape[1] != 3:
+        return False  # 1-channel features broadcast in the reference
+    n = len(meshes)
+    for owner, names in ((lights, ("ambient_color", "diffuse_color", "specular_color", "location", "direction")),
+                         (materials, ("ambient_color", "diffuse_color", "specular_color", "shininess"))):
+        for name in names:
+            t = getattr(owner, name, None)
+            if t is None:
+                continue
+            if not torch.is_tensor(t) or t.dim() < 1 or t.shape[0] not in (1, n):
+                return False
+            if name != "shininess" and (t.dim() != 2 or t.shape[-1] != 3):
+                return False
+    for name in ("R", "T"):  # the camera batch: the fused op forms one camera centre per mesh
+        t = getattr(cameras, name, None)
+        if not torch.is_tensor(t) or t.dim() < 1 or t.shape[0] not in (1, n):
+            return False
+    return True
+
+
+def _gouraud_dispatch(original):
+    from . import shading as ours
+
+    def gouraud_shading(meshes, fragments, lights, cameras, materials):
+        if _gouraud_fused(meshes, fragments, lights, cameras, materials):
+            return ours.gouraud_shading(meshes, fragments, lights, cameras, materials)
+        return original(meshes, fragments, lights, cameras, materials)
+
+    gouraud_shading.__doc__ = original.__doc__
+    return gouraud_shading
+
+
+def install_gouraud():
+    """Patch PyTorch3D's Gouraud shading (must be importable): `gouraud_shading` in pytorch3d.renderer.mesh.shading and
+    in pytorch3d.renderer.mesh.shader, which imports it by name.  Returns the list of patched module names."""
+    for modname in _SHADING_MODULES:
+        m = importlib.import_module(modname)
+        if (modname, "gouraud_shading") not in _saved_blend and hasattr(m, "gouraud_shading"):
+            _saved_blend[(modname, "gouraud_shading")] = m.gouraud_shading
+            m.gouraud_shading = _gouraud_dispatch(m.gouraud_shading)
+    return list(_SHADING_MODULES)
+
+
 def _textures_fused(textures, fragments):
     """Whether the fused texture sampling takes this call: one map per mesh, a non-empty texture, float32 CUDA maps and
     barycentrics and int64 CUDA pix_to_face on one device, a sampling and padding mode the kernels implement, one map per
@@ -393,8 +470,8 @@ def install_clipping():
 
 
 def uninstall():
-    """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_textures()`,
-    `install_texture_atlas()` and `install_clipping()`."""
+    """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_gouraud()`,
+    `install_textures()`, `install_texture_atlas()` and `install_clipping()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original

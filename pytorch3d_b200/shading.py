@@ -1,5 +1,6 @@
-"""Phong and flat shading, same API as the reference's pytorch3d/renderer/mesh/shading.py: `phong_shading`,
-`_phong_shading_with_pixels` and `flat_shading`, with the light models of pytorch3d/renderer/lighting.py.
+"""Phong, flat and Gouraud shading, same API as the reference's pytorch3d/renderer/mesh/shading.py: `phong_shading`,
+`_phong_shading_with_pixels`, `flat_shading` and `gouraud_shading`, with the light models of
+pytorch3d/renderer/lighting.py.
 
 Each slot's position and normal are interpolated from its face (phong) or taken from the face (flat) and lit by one
 point, directional or ambient light; the colour is `(ambient + diffuse) * texel + specular`.  The reference writes about
@@ -11,6 +12,10 @@ Objects are duck-typed.  `meshes` needs `verts_packed`, `faces_packed` and `vert
 `diffuse_color`, `specular_color` and `shininess`.  A light with a `location` is a point light, one with a `direction`
 a directional light, and one with neither an ambient light.  Gradients reach the texels, the barycentric coordinates,
 the vertices and normals, and every light, material and camera tensor.
+
+`gouraud_shading` lights every vertex instead (one kernel), then interpolates the shaded vertex colours at the slots
+(a second one), with no (F, 3, 3) gather (DESIGN.md section 16).  Its `meshes` also needs `textures` with
+`verts_features_packed`, `num_verts_per_mesh` and `mesh_to_verts_packed_first_idx`; its parameter rows are per mesh.
 """
 from typing import Tuple
 
@@ -18,7 +23,7 @@ import torch
 
 from . import _C
 
-__all__ = ["phong_shading", "_phong_shading_with_pixels", "flat_shading", "light_kind"]
+__all__ = ["phong_shading", "_phong_shading_with_pixels", "flat_shading", "gouraud_shading", "light_kind"]
 
 
 class _Shading(torch.autograd.Function):
@@ -59,11 +64,12 @@ def _rows(name, x, width, device):
     return t
 
 
-def _params(N, lights, cameras, materials, kind, device):
-    """The per-image parameter row (N, 22) of the shading kernels, with the reference's batch rules: every piece has
-    batch 1 or N (ValueError "Got non-broadcastable sizes" otherwise).  `ambient` is formed as the reference forms it,
-    `materials.ambient_color * lights.ambient_color`; autograd returns each piece's gradient to its source, summed over
-    the batch where the source has batch 1."""
+def _params(N, lights, cameras, materials, kind, device, batched_material_colors=False):
+    """The per-image (per-mesh for Gouraud) parameter row (N, 22) of the shading kernels, with the reference's batch
+    rules: every piece has batch 1 or N (ValueError "Got non-broadcastable sizes" otherwise).  `ambient` is formed as
+    the reference forms it, `materials.ambient_color * lights.ambient_color`; autograd returns each piece's gradient to
+    its source, summed over the batch where the source has batch 1.  Material diffuse and specular colours must have
+    batch 1 unless `batched_material_colors` (Gouraud shading, where the reference gathers them per vertex)."""
     ambient = _rows("ambient_color", materials.ambient_color * lights.ambient_color, 3, device)
     md = _rows("diffuse_color", materials.diffuse_color, 3, device)
     ms = _rows("specular_color", materials.specular_color, 3, device)
@@ -82,7 +88,7 @@ def _params(N, lights, cameras, materials, kind, device):
     sizes = [N] + [int(p.shape[0]) for p in pieces]
     if any(s not in (1, N) for s in sizes):
         raise ValueError("Got non-broadcastable sizes %r" % sizes)
-    if md.shape[0] != 1 or ms.shape[0] != 1:
+    if not batched_material_colors and (md.shape[0] != 1 or ms.shape[0] != 1):
         # the reference multiplies these (B, 3) colours into the (N, H, W, K, 3) light colours, which only broadcasts
         # for B = 1
         raise ValueError("Got non-broadcastable sizes %r: material diffuse and specular colours must have batch 1"
@@ -133,3 +139,40 @@ def flat_shading(meshes, fragments, lights, cameras, materials, texels) -> torch
     N = int(fragments.pix_to_face.shape[0])
     params = _params(N, lights, cameras, materials, kind, texels.device)
     return _Shading.apply(texels, None, face_coords, face_normals, params, fragments.pix_to_face, True, kind, False)
+
+
+class _Gouraud(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, verts, normals, verts_colors, bary, params, first, num, faces, pix_to_face, light):
+        colors, shaded = _C.gouraud_forward(verts, normals, verts_colors, first, num, params, faces, pix_to_face, bary,
+                                            light)
+        ctx.save_for_backward(verts, normals, verts_colors, bary, params, first, num, faces, pix_to_face, shaded)
+        ctx.light = light
+        return colors
+
+    @staticmethod
+    def backward(ctx, grad_colors):
+        verts, normals, verts_colors, bary, params, first, num, faces, pix_to_face, shaded = ctx.saved_tensors
+        grads = _C.gouraud_backward(grad_colors.contiguous(), verts, normals, verts_colors, first, num, params, faces,
+                                    pix_to_face, bary, ctx.light, shaded, ctx.needs_input_grad[:5])
+        return grads + (None, None, None, None, None)
+
+
+def gouraud_shading(meshes, fragments, lights, cameras, materials) -> torch.Tensor:
+    """Per-vertex shading: every vertex lit with its mesh's lights, camera and material, its colour
+    `verts_colors * (ambient + diffuse) + specular`, then interpolated with the barycentric coordinates.  The vertex
+    colours come from a `TexturesVertex` with 3 channels.  -> colors (N,H,W,K,3)."""
+    textures = getattr(meshes, "textures", None)
+    if not hasattr(textures, "verts_features_packed"):
+        raise ValueError("Mesh textures must be an instance of TexturesVertex")
+    verts, faces = meshes.verts_packed(), meshes.faces_packed()
+    verts_colors = textures.verts_features_packed()
+    if tuple(verts_colors.shape) != (verts.shape[0], 3):
+        raise ValueError("Gouraud shading needs vertex colours of shape (V, 3) = %r; got %r"
+                         % ((int(verts.shape[0]), 3), tuple(verts_colors.shape)))
+    kind = light_kind(lights)
+    normals = None if kind == "ambient" else meshes.verts_normals_packed()
+    params = _params(len(meshes), lights, cameras, materials, kind, verts.device, batched_material_colors=True)
+    return _Gouraud.apply(verts, normals, verts_colors, fragments.bary_coords, params,
+                          meshes.mesh_to_verts_packed_first_idx(), meshes.num_verts_per_mesh(), faces,
+                          fragments.pix_to_face, kind)

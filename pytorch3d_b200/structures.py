@@ -33,6 +33,8 @@ class PackedMeshes:
         if self._N > 1:
             first[1:] = torch.cumsum(self._num_faces_per_mesh, 0)[:-1]
         self._mesh_to_faces_packed_first_idx = first
+        self._num_verts_per_mesh = torch.tensor(v_counts, dtype=torch.int64, device=self.device)
+        self._mesh_to_verts_packed_first_idx = torch.tensor(v_off, dtype=torch.int64, device=self.device)
         self._F = max(f_counts) if f_counts else 0
         self._V = max(v_counts) if v_counts else 0
 
@@ -50,6 +52,12 @@ class PackedMeshes:
 
     def num_faces_per_mesh(self):
         return self._num_faces_per_mesh
+
+    def num_verts_per_mesh(self):
+        return self._num_verts_per_mesh
+
+    def mesh_to_verts_packed_first_idx(self):
+        return self._mesh_to_verts_packed_first_idx
 
     def isempty(self):
         return self._N == 0 or self._verts_packed.shape[0] == 0
