@@ -422,6 +422,38 @@ int b200r_texture_atlas_backward(const float* grad_texels, const int64_t* pix_to
                                  float* grad_atlas, void* stream);
 
 /*
+ * Mesh normals (DESIGN.md section 17).  verts float32 (V,3) and faces int64 (F,3), contiguous, read in place (64-bit
+ * offsets); V < 2^31 - 1 and 3F < 2^31, larger sizes return B200R_ERR_INVALID_ARGUMENT.  A face index outside [0, V)
+ * (the reference does not check them) gives NaN for that face and belongs to no vertex.  All entry points are
+ * asynchronous, use no float atomics and are deterministic.
+ *
+ * The vertex -> corner table: int32, V + 1 offsets followed by the 3F corner ids j * F + f sorted by their vertex
+ * faces[f, j] (stable, so in (j, f) order within a vertex).  Vertex v's corners are ids[offsets[v] .. offsets[v+1]).
+ *
+ * face_areas_normals_forward / _backward: pytorch3d._C's ops of these names (face_areas_normals.h), for float32.  The
+ *  forward writes areas (F,) and normals (F,3), bit-identical to the reference's CUDA kernel built for sm_90a.  The
+ *  backward takes grad_areas (F,) and grad_normals (F,3) float32, contiguous, and writes grad_verts (V,3): the
+ *  reference's per-corner terms summed per vertex in the table's order (the table is built in the call).
+ * verts_normals_forward: what pytorch3d.structures.Meshes._compute_vertex_normals computes, bit-identical to it on the
+ *  CPU: normals (V,3) = s / max(|s|, 1e-6), s the sum of (v2 - v1) x (v0 - v1) over the vertex's corners.  Also writes
+ *  the table (V + 1 + 3F ints) and s (V,3) float32, which the backward reads.
+ * verts_normals_backward: grad_normals float32 (V,3), contiguous -> grad_verts (V,3), autograd's gradient of that chain.
+ * workspace: b200r_normals_workspace_bytes(V, F) bytes for any of the three entry points that take one, a function of
+ *  the shapes only; it allocates and launches nothing (0 when there is no device to size the sort for).
+ */
+size_t b200r_normals_workspace_bytes(int64_t V, int64_t F);
+int b200r_face_areas_normals_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F, float* areas,
+                                     float* normals, void* stream);
+int b200r_face_areas_normals_backward(const float* grad_areas, const float* grad_normals, const float* verts,
+                                      int64_t V, const int64_t* faces, int64_t F, void* workspace,
+                                      size_t workspace_bytes, float* grad_verts, void* stream);
+int b200r_verts_normals_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F, void* workspace,
+                                size_t workspace_bytes, int32_t* table, float* sums, float* normals, void* stream);
+int b200r_verts_normals_backward(const float* grad_normals, const float* verts, int64_t V, const int64_t* faces,
+                                 int64_t F, const int32_t* table, const float* sums, void* workspace,
+                                 size_t workspace_bytes, float* grad_verts, void* stream);
+
+/*
  * Fused frustum culling and z-clipping (additional entry points, no counterpart in pytorch3d._C): what
  * pytorch3d/renderer/mesh/clip.py clip_faces and convert_clipped_rasterization_to_original_faces compute, with the
  * reference's output layout (DESIGN.md section 14).  All entry points are asynchronous.

@@ -960,6 +960,122 @@ def texture_atlas_backward(grad_texels: torch.Tensor, pix_to_face: torch.Tensor,
     return grad_atlas
 
 
+def normals_key_bits(V: int):
+    """The key bits of the vertex -> corner table's sort: vertex ids and the key V (faces out of range) need
+    ceil(log2(V + 1)) bits, at least 1 (b200r_normals_workspace_bytes)."""
+    return max(1, int(V).bit_length())
+
+
+def normals_table_size(V: int, F: int):
+    """Entries (int32) of the vertex -> corner table: V + 1 offsets, then the 3F corner ids."""
+    return int(V) + 1 + 3 * int(F)
+
+
+def _check_mesh_inputs(op, verts, faces):
+    """(V, F, device) of float32 verts (V, 3) and int64 faces (F, 3) on one CUDA device; raises RuntimeError otherwise,
+    and for sizes past the kernels' limits (V < 2^31 - 1, 3F < 2^31)."""
+    dev = _require_cuda(("verts", verts), ("faces", faces))
+    if verts.dtype != torch.float32:
+        raise RuntimeError("%s: expected scalar type Float for verts but found %s" % (op, verts.dtype))
+    if faces.dtype != torch.int64:
+        raise RuntimeError("%s: expected scalar type Long for faces but found %s" % (op, faces.dtype))
+    if verts.dim() != 2 or verts.shape[1] != 3:
+        raise RuntimeError("%s: verts must be (V, 3), got %s" % (op, tuple(verts.shape)))
+    if faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError("%s: faces must be (F, 3), got %s" % (op, tuple(faces.shape)))
+    V, F = int(verts.shape[0]), int(faces.shape[0])
+    if V >= (1 << 31) - 1 or 3 * F >= (1 << 31):
+        raise RuntimeError("%s: at most 2^31 - 2 vertices and (2^31 - 1) / 3 faces, got V = %d, F = %d" % (op, V, F))
+    return V, F, dev
+
+
+def _check_grad(name, t, shape, dev):
+    _require_cuda((name, t))
+    if t.device != dev:
+        raise RuntimeError("Expected all tensors to be on the same device (%s is on %s, expected %s)"
+                           % (name, t.device, dev))
+    if t.dtype != torch.float32 or tuple(t.shape) != tuple(shape):
+        raise RuntimeError("%s must be a float32 tensor of shape %s, got %s %s"
+                           % (name, tuple(shape), t.dtype, tuple(t.shape)))
+    return t.contiguous()
+
+
+def _normals_workspace(lib, V, F, dev):
+    ws_bytes = int(lib.b200r_normals_workspace_bytes(V, F))
+    return torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None, ws_bytes  # 512-byte aligned
+
+
+def face_areas_normals_forward(verts: torch.Tensor, faces: torch.Tensor):
+    """pytorch3d._C.face_areas_normals_forward (FaceAreasNormalsForward, csrc/face_areas_normals/face_areas_normals.h)
+    for float32: verts (V,3) f32, faces (F,3) i64 -> (areas (F,) f32, normals (F,3) f32), bit-identical to the
+    reference's CUDA kernel."""
+    V, F, dev = _check_mesh_inputs("face_areas_normals_forward", verts, faces)
+    lib = _lib.load()
+    v, f = verts.contiguous(), faces.contiguous()
+    with torch.cuda.device(dev):
+        areas = torch.empty((F,), dtype=torch.float32, device=dev)
+        normals = torch.empty((F, 3), dtype=torch.float32, device=dev)
+        _lib.check(lib.b200r_face_areas_normals_forward(_ptr(v), V, _ptr(f), F, _ptr(areas), _ptr(normals),
+                                                        _stream_ptr(dev)))
+    return areas, normals
+
+
+def face_areas_normals_backward(grad_areas: torch.Tensor, grad_normals: torch.Tensor, verts: torch.Tensor,
+                                faces: torch.Tensor):
+    """pytorch3d._C.face_areas_normals_backward (FaceAreasNormalsBackward) for float32 -> grad_verts (V,3) f32: the
+    reference's per-corner gradients, summed per vertex in a fixed order.  Deterministic (no atomics), so unlike the
+    reference it runs under torch.use_deterministic_algorithms(True)."""
+    V, F, dev = _check_mesh_inputs("face_areas_normals_backward", verts, faces)
+    ga = _check_grad("grad_areas", grad_areas, (F,), dev)
+    gn = _check_grad("grad_normals", grad_normals, (F, 3), dev)
+    lib = _lib.load()
+    v, f = verts.contiguous(), faces.contiguous()
+    with torch.cuda.device(dev):
+        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        ws, ws_bytes = _normals_workspace(lib, V, F, dev)
+        _lib.check(lib.b200r_face_areas_normals_backward(_ptr(ga), _ptr(gn), _ptr(v), V, _ptr(f), F, _ptr(ws),
+                                                         ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
+    return grad_verts
+
+
+def verts_normals_forward(verts: torch.Tensor, faces: torch.Tensor):
+    """Fused Meshes._compute_vertex_normals (no counterpart in pytorch3d._C; DESIGN.md section 17): verts (V,3) f32,
+    faces (F,3) i64 -> (normals (V,3) f32, table (V + 1 + 3F,) i32, sums (V,3) f32).  The normals are bit-identical to
+    the reference's torch chain on the CPU; the table and the unnormalised sums are what `verts_normals_backward`
+    reads."""
+    V, F, dev = _check_mesh_inputs("verts_normals_forward", verts, faces)
+    lib = _lib.load()
+    v, f = verts.contiguous(), faces.contiguous()
+    with torch.cuda.device(dev):
+        normals = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        table = torch.empty((normals_table_size(V, F),), dtype=torch.int32, device=dev)
+        sums = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        ws, ws_bytes = _normals_workspace(lib, V, F, dev)
+        _lib.check(lib.b200r_verts_normals_forward(_ptr(v), V, _ptr(f), F, _ptr(ws), ws_bytes, _ptr(table),
+                                                   _ptr(sums), _ptr(normals), _stream_ptr(dev)))
+    return normals, table, sums
+
+
+def verts_normals_backward(grad_normals: torch.Tensor, verts: torch.Tensor, faces: torch.Tensor, table: torch.Tensor,
+                           sums: torch.Tensor):
+    """Backward of `verts_normals_forward` -> grad_verts (V,3) f32, from the forward's table and sums (no sort).
+    Deterministic, no atomics; nothing synchronises the host."""
+    V, F, dev = _check_mesh_inputs("verts_normals_backward", verts, faces)
+    gn = _check_grad("grad_normals", grad_normals, (V, 3), dev)
+    s = _check_grad("sums", sums, (V, 3), dev)
+    _require_cuda(("table", table))
+    if table.device != dev or table.dtype != torch.int32 or tuple(table.shape) != (normals_table_size(V, F),):
+        raise RuntimeError("table must be the int32 (V + 1 + 3F,) table of verts_normals_forward on %s" % dev)
+    lib = _lib.load()
+    v, f, t = verts.contiguous(), faces.contiguous(), table.contiguous()
+    with torch.cuda.device(dev):
+        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        ws, ws_bytes = _normals_workspace(lib, V, F, dev)
+        _lib.check(lib.b200r_verts_normals_backward(_ptr(gn), _ptr(v), V, _ptr(f), F, _ptr(t), _ptr(s), _ptr(ws),
+                                                    ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
+    return grad_verts
+
+
 def _clip_frustum_args(frustum):
     """(planes (6,) float32 host array, cull_mask, has_z_clip, z_clip, perspective_correct) of a ClipFrustum-like
     object for the b200r_clip_* entry points."""

@@ -98,6 +98,11 @@ SIGNATURES = {
         ctypes.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "b200r_texture_atlas_backward": (
         ctypes.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp, _vp]),
+    "b200r_normals_workspace_bytes": (_sz, [_i64, _i64]),
+    "b200r_face_areas_normals_forward": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _vp]),
+    "b200r_face_areas_normals_backward": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
+    "b200r_verts_normals_forward": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "b200r_verts_normals_backward": (ctypes.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _sz, _vp, _vp]),
     "b200r_clip_faces_workspace_words": (_i64, [_i64]),
     "b200r_clip_faces_count": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i32, _i32, _f64, _vp, _vp]),
     "b200r_clip_faces_fill": (

@@ -1,0 +1,459 @@
+// Mesh normals: vertex normals and face areas / normals, forward and deterministic backward (DESIGN.md section 17).
+//
+// Both ops rest on one structure, the vertex -> corner table.  Corner j of face f has the id c = j * F + f and the key
+// faces[f, j]; a stable radix sort of the 3F (key, id) pairs over ceil(log2(V + 1)) key bits, and an offset array of
+// V + 1 entries, give every vertex the run of its corners in (j, f) order.  That is the order in which the three
+// serial index_add calls of pytorch3d/structures/meshes.py Meshes._compute_vertex_normals accumulate on the CPU.  Every
+// per-vertex sum is one thread walking its run from +0 with __fadd_rn (segmented_sum_kernel, shared by both ops), so
+// there are no float atomics and the results do not depend on scheduling.  Nothing synchronises the host, and the
+// workspace depends only on (V, F).
+//
+// Vertex normals (Meshes._compute_vertex_normals, restated with explicit rounding):
+//   n_f = (v2 - v1) x (v0 - v1), each component fma(a_i, b_j, -rn(a_j * b_i)) with a = v2 - v1, b = v0 - v1
+//   s_v = the sum of n_f over the corners of v, in (j, f) order from +0
+//   out = s_v / max(|s_v|, 1e-6), |s| = sqrt_rn(fma(z, z, fma(y, y, rn(x * x)))), an IEEE divide
+// The backward is autograd's through F.normalize (x / clamp_min(norm, eps)), the cross product and the two
+// subtractions, with the per-corner gradients summed per vertex over the forward's table.
+//
+// Face areas and normals (pytorch3d/csrc/face_areas_normals/face_areas_normals.cu): the forward restates
+// FaceAreasNormalsForwardKernel<float> as nvcc compiles it for sm_90a (its FMA contraction, the double compare against
+// 1e-6, norm / 2.0), so the results are bit-identical.  The backward writes the reference's nine per-corner expressions,
+// in its arithmetic, to an (F, 3, 3) workspace, and sums them per vertex over a table built in the same call instead of
+// adding them with float atomics.
+#include <cub/device/device_radix_sort.cuh>
+
+#include "common.cuh"
+
+namespace b200r {
+namespace {
+
+constexpr int kThreads = 256;
+constexpr float kNormalizeEps = 1e-6f;  // F.normalize(..., eps=1e-6) in Meshes._compute_vertex_normals
+constexpr size_t kAlign = 256;
+
+// The three corners of face f.  A face index outside [0, V) (the reference does not check them either) gives NaN
+// corners instead of a read out of bounds.
+__device__ __forceinline__ void face_corners(const float* __restrict__ verts, const int64_t* __restrict__ faces,
+                                             int64_t V, int64_t f, float3 p[3]) {
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const int64_t v = __ldg(faces + 3 * f + j);
+    if (v >= 0 && v < V) {
+      p[j] = make_float3(__ldg(verts + 3 * v + 0), __ldg(verts + 3 * v + 1), __ldg(verts + 3 * v + 2));
+    } else {
+      const float nan = __int_as_float(0x7fc00000);
+      p[j] = make_float3(nan, nan, nan);
+    }
+  }
+}
+
+__device__ __forceinline__ float3 sub_rn(float3 a, float3 b) {
+  return make_float3(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z));
+}
+
+// a x b with each component fma(a_i, b_j, -rn(a_j * b_i)): torch.cross on float32 as compiled for the CPU, and autograd's
+// cross backward.
+__device__ __forceinline__ float3 cross_fma(float3 a, float3 b) {
+  return make_float3(__fmaf_rn(a.y, b.z, -__fmul_rn(a.z, b.y)), __fmaf_rn(a.z, b.x, -__fmul_rn(a.x, b.z)),
+                     __fmaf_rn(a.x, b.y, -__fmul_rn(a.y, b.x)));
+}
+
+// |s| as torch's 2-norm over dim 1 of a float32 (V, 3) tensor computes it.
+__device__ __forceinline__ float norm3(float3 s) {
+  return __fsqrt_rn(__fmaf_rn(s.z, s.z, __fmaf_rn(s.y, s.y, __fmul_rn(s.x, s.x))));
+}
+
+__device__ __forceinline__ float3 load3(const float* __restrict__ p, int64_t i) {
+  return make_float3(__ldg(p + 3 * i + 0), __ldg(p + 3 * i + 1), __ldg(p + 3 * i + 2));
+}
+
+__device__ __forceinline__ void store3(float* __restrict__ p, int64_t i, float3 v) {
+  p[3 * i + 0] = v.x;
+  p[3 * i + 1] = v.y;
+  p[3 * i + 2] = v.z;
+}
+
+// ---- the vertex -> corner table ---------------------------------------------------------------------------------
+
+// (key, corner id) of every corner; a face index outside [0, V) gets the key V, which sorts after every vertex and
+// belongs to no run.
+__global__ void __launch_bounds__(kThreads)
+    corner_keys_kernel(const int64_t* __restrict__ faces, int64_t F, int64_t V, uint32_t* __restrict__ keys,
+                       int32_t* __restrict__ ids) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += stride) {
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const int64_t v = __ldg(faces + 3 * f + j);
+      const int64_t c = j * F + f;
+      keys[c] = (uint32_t)((v >= 0 && v < V) ? v : V);
+      ids[c] = (int32_t)c;
+    }
+  }
+}
+
+// offsets[v] = the first sorted position whose key is >= v, for v in [0, V]: position i writes the offsets of the
+// vertices after the previous key up to its own (the end, n, stands for the key V).
+__global__ void __launch_bounds__(kThreads)
+    run_offsets_kernel(const uint32_t* __restrict__ keys, int64_t n, int64_t V, int32_t* __restrict__ offsets) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += stride) {
+    const int64_t prev = i > 0 ? (int64_t)keys[i - 1] : -1;
+    const int64_t cur = i < n ? (int64_t)keys[i] : V;
+    for (int64_t v = prev + 1; v <= cur; ++v) offsets[v] = (int32_t)i;
+  }
+}
+
+// ---- the one segmented sum --------------------------------------------------------------------------------------
+
+enum class RowOf { kFace, kCorner };   // rows[f] (F, 3) or rows[f * 3 + j] (F, 3, 3)
+enum class Epilogue { kSum, kNormalize };
+
+// Per vertex: the sum of its corners' rows in run order from +0.  kNormalize also stores the sum in `sums` and writes
+// sum / max(|sum|, 1e-6) to `out`.
+template <RowOf ROW, Epilogue EPI>
+__global__ void __launch_bounds__(kThreads)
+    segmented_sum_kernel(const int32_t* __restrict__ offsets, const int32_t* __restrict__ corners, int64_t V,
+                         int64_t F, const float* __restrict__ rows, float* __restrict__ sums,
+                         float* __restrict__ out) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < V; v += stride) {
+    const int32_t end = __ldg(offsets + v + 1);
+    float3 acc = make_float3(0.0f, 0.0f, 0.0f);
+    for (int32_t i = __ldg(offsets + v); i < end; ++i) {
+      const int64_t c = __ldg(corners + i);
+      const int64_t j = c >= 2 * F ? 2 : (c >= F ? 1 : 0);
+      const int64_t f = c - j * F;
+      const float3 r = load3(rows, ROW == RowOf::kFace ? f : f * 3 + j);
+      acc = make_float3(__fadd_rn(acc.x, r.x), __fadd_rn(acc.y, r.y), __fadd_rn(acc.z, r.z));
+    }
+    if (EPI == Epilogue::kNormalize) {
+      store3(sums, v, acc);
+      const float n = norm3(acc);
+      const float m = n < kNormalizeEps ? kNormalizeEps : n;  // clamp_min: NaN stays NaN
+      acc = make_float3(__fdiv_rn(acc.x, m), __fdiv_rn(acc.y, m), __fdiv_rn(acc.z, m));
+    }
+    store3(out, v, acc);
+  }
+}
+
+// ---- vertex normals -----------------------------------------------------------------------------------------------
+
+__global__ void __launch_bounds__(kThreads)
+    face_normal_rows_kernel(const float* __restrict__ verts, const int64_t* __restrict__ faces, int64_t V, int64_t F,
+                            float* __restrict__ rows) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += stride) {
+    float3 p[3];
+    face_corners(verts, faces, V, f, p);
+    store3(rows, f, cross_fma(sub_rn(p[2], p[1]), sub_rn(p[0], p[1])));
+  }
+}
+
+// d loss / d s for y = s / clamp_min(|s|, eps), as autograd forms it: the quotient's two gradients, clamp_min's
+// (none below eps), and the norm's (none where |s| = 0).
+__global__ void __launch_bounds__(kThreads)
+    normalize_backward_kernel(const float* __restrict__ grad_normals, const float* __restrict__ sums, int64_t V,
+                              float* __restrict__ grad_sums) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < V; v += stride) {
+    const float3 s = load3(sums, v), g = load3(grad_normals, v);
+    const float n = norm3(s);
+    const float m = n < kNormalizeEps ? kNormalizeEps : n;
+    // div's gradient to the divisor, -g * ((s / m) / m), summed over the three components by expand_as's backward
+    const float gm = __fadd_rn(__fadd_rn(-__fmul_rn(g.x, __fdiv_rn(__fdiv_rn(s.x, m), m)),
+                                         -__fmul_rn(g.y, __fdiv_rn(__fdiv_rn(s.y, m), m))),
+                               -__fmul_rn(g.z, __fdiv_rn(__fdiv_rn(s.z, m), m)));
+    const float gn = n >= kNormalizeEps ? gm : 0.0f;     // clamp_min(norm, eps): where(norm >= eps, grad, 0)
+    const float k = n == 0.0f ? 0.0f : __fdiv_rn(gn, n);  // the norm's backward: s * (grad / norm), 0 where norm == 0
+    store3(grad_sums, v,
+           make_float3(__fadd_rn(__fdiv_rn(g.x, m), __fmul_rn(s.x, k)), __fadd_rn(__fdiv_rn(g.y, m), __fmul_rn(s.y, k)),
+                       __fadd_rn(__fdiv_rn(g.z, m), __fmul_rn(s.z, k))));
+  }
+}
+
+// Per face: the gradient of n_f (the sum of grad_sums over its three corners), through the cross product and the two
+// subtractions, as rows (f, j) = d loss / d corner j.
+__global__ void __launch_bounds__(kThreads)
+    cross_backward_rows_kernel(const float* __restrict__ verts, const int64_t* __restrict__ faces, int64_t V,
+                               int64_t F, const float* __restrict__ grad_sums, float* __restrict__ rows) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += stride) {
+    float3 p[3];
+    face_corners(verts, faces, V, f, p);
+    float3 gs = make_float3(0.0f, 0.0f, 0.0f);
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const int64_t v = __ldg(faces + 3 * f + j);
+      const float3 g = (v >= 0 && v < V) ? load3(grad_sums, v) : make_float3(0.0f, 0.0f, 0.0f);
+      gs = make_float3(__fadd_rn(gs.x, g.x), __fadd_rn(gs.y, g.y), __fadd_rn(gs.z, g.z));
+    }
+    const float3 a = sub_rn(p[2], p[1]), b = sub_rn(p[0], p[1]);
+    const float3 ga = cross_fma(b, gs);  // cross(a, b) backward: a gets b x g, b gets g x a
+    const float3 gb = cross_fma(gs, a);
+    store3(rows, f * 3 + 0, gb);
+    store3(rows, f * 3 + 1,
+           make_float3(__fsub_rn(-ga.x, gb.x), __fsub_rn(-ga.y, gb.y), __fsub_rn(-ga.z, gb.z)));
+    store3(rows, f * 3 + 2, ga);
+  }
+}
+
+// ---- face areas and normals ---------------------------------------------------------------------------------------
+
+// FaceAreasNormalsForwardKernel<float> as nvcc compiles it for sm_90a: each cross component is FFMA(first product,
+// -FMUL(second product)), the squared norm FFMA(cz, cz, FFMA(cx, cx, FMUL(cy, cy))), then an IEEE square root.  The
+// area norm / 2.0, formed in double and rounded to float, is exactly FMUL(norm, 0.5).  The clamp compares in double
+// (NaN passes) and clamps to (float)1e-6; the normal is an IEEE divide.
+__global__ void __launch_bounds__(kThreads)
+    face_areas_normals_forward_kernel(const float* __restrict__ verts, const int64_t* __restrict__ faces, int64_t V,
+                                      int64_t F, float* __restrict__ areas, float* __restrict__ normals) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += stride) {
+    float3 p[3];
+    face_corners(verts, faces, V, f, p);
+    const float3 a = sub_rn(p[1], p[0]), b = sub_rn(p[2], p[0]);
+    const float cx = __fmaf_rn(a.y, b.z, -__fmul_rn(a.z, b.y));
+    const float cy = __fmaf_rn(a.z, b.x, -__fmul_rn(a.x, b.z));
+    const float cz = __fmaf_rn(a.x, b.y, -__fmul_rn(a.y, b.x));
+    float norm = __fsqrt_rn(__fmaf_rn(cz, cz, __fmaf_rn(cx, cx, __fmul_rn(cy, cy))));
+    areas[f] = __fmul_rn(norm, 0.5f);
+    norm = ((double)norm < 1e-6) ? (float)1e-6 : norm;
+    store3(normals, f, make_float3(__fdiv_rn(cx, norm), __fdiv_rn(cy, norm), __fdiv_rn(cz, norm)));
+  }
+}
+
+// The reference backward's per-corner expressions (FaceAreasNormalsBackwardKernel), in its arithmetic: float
+// products, the area term divided by 2.0 in double, pow() for the inverse norm's powers, and the sum of the four terms
+// rounded to float once.  Row (f, j) = the gradient of corner j.
+__global__ void __launch_bounds__(kThreads)
+    face_areas_normals_backward_rows_kernel(const float* __restrict__ grad_areas,
+                                            const float* __restrict__ grad_normals, const float* __restrict__ verts,
+                                            const int64_t* __restrict__ faces, int64_t V, int64_t F,
+                                            float* __restrict__ rows) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += stride) {
+    float3 p[3];
+    face_corners(verts, faces, V, f, p);
+    const float ax = p[1].x - p[0].x, ay = p[1].y - p[0].y, az = p[1].z - p[0].z;
+    const float bx = p[2].x - p[0].x, by = p[2].y - p[0].y, bz = p[2].z - p[0].z;
+    const float cx = ay * bz - az * by;
+    const float cy = az * bx - ax * bz;
+    const float cz = ax * by - ay * bx;
+    float norm = sqrtf(cx * cx + cy * cy + cz * cz);
+    norm = (norm < 1e-6) ? 1e-6 : norm;
+    const float inv = 1. / norm;
+    const float inv2 = powf(inv, 2.0f);
+    const float inv3 = powf(inv, 3.0f);
+    const float ga = __ldg(grad_areas + f);
+    const float g0 = __ldg(grad_normals + 3 * f + 0), g1 = __ldg(grad_normals + 3 * f + 1),
+                g2 = __ldg(grad_normals + 3 * f + 2);
+    // t is d(c)/d(coordinate) . c; each component's gradient is
+    //   t / 2.0 * inv * ga + sum_k (term of normal component k)
+    // where the component of c that the coordinate does not move gets -c_k * t * inv3 * g_k and the other two
+    // (d_k - c_k * t * inv2) * inv * g_k, each written out as the reference writes it.
+    float* r = rows + 9 * f;
+    float t;
+    // corner 0
+    t = (-az + bz) * cy + (-by + ay) * cz;
+    r[0] = t / 2.0 * inv * ga + -cx * t * inv3 * g0 + ((-az + bz) - cy * t * inv2) * inv * g1 +
+           ((-by + ay) - cz * t * inv2) * inv * g2;
+    t = (-bz + az) * cx + (-ax + bx) * cz;
+    r[1] = t / 2.0 * inv * ga + ((-bz + az) - cx * t * inv2) * inv * g0 + -cy * t * inv3 * g1 +
+           ((-ax + bx) - cz * t * inv2) * inv * g2;
+    t = (-ay + by) * cx + (-bx + ax) * cy;
+    r[2] = t / 2.0 * inv * ga + ((-ay + by) - cx * t * inv2) * inv * g0 + ((-bx + ax) - cy * t * inv2) * inv * g1 +
+           -cz * t * inv3 * g2;
+    // corner 1
+    t = by * cz - bz * cy;
+    r[3] = t / 2.0 * inv * ga + -cx * t * inv3 * g0 + (-bz - cy * t * inv2) * inv * g1 + (by - cz * t * inv2) * inv * g2;
+    t = bz * cx - bx * cz;
+    r[4] = t / 2.0 * inv * ga + (bz - cx * t * inv2) * inv * g0 + -cy * t * inv3 * g1 + (-bx - cz * t * inv2) * inv * g2;
+    t = bx * cy - by * cx;
+    // the reference multiplies the second normal component's term by cx, not cy; kept, the records depend on it
+    r[5] = t / 2.0 * inv * ga + (-by - cx * t * inv2) * inv * g0 + (bx - cx * t * inv2) * inv * g1 + -cz * t * inv3 * g2;
+    // corner 2
+    t = az * cy - ay * cz;
+    r[6] = t / 2.0 * inv * ga + -cx * t * inv3 * g0 + (az - cy * t * inv2) * inv * g1 + (-ay - cz * t * inv2) * inv * g2;
+    t = ax * cz - az * cx;
+    r[7] = t / 2.0 * inv * ga + (-az - cx * t * inv2) * inv * g0 + -cy * t * inv3 * g1 + (ax - cz * t * inv2) * inv * g2;
+    t = ay * cx - ax * cy;
+    r[8] = t / 2.0 * inv * ga + (ay - cx * t * inv2) * inv * g0 + (-ax - cy * t * inv2) * inv * g1 + -cz * t * inv3 * g2;
+  }
+}
+
+// ---- host side ----------------------------------------------------------------------------------------------------
+
+// ceil(log2(V + 1)): the key bits the sort looks at (the key V, for faces out of range, included).
+int key_bits(int64_t V) {
+  int bits = 1;
+  while (bits < 32 && (V >> bits) != 0) ++bits;
+  return bits;
+}
+
+// Workspace: rows (9F floats), a table (V + 1 + 3F ints), keys in / out and ids (3F each), then cub's temporary
+// storage.  Returns false when cub cannot size its storage (no device).
+struct Layout {
+  size_t rows, table, keys_in, keys_out, ids_in, cub, cub_bytes, total;
+};
+
+bool layout(int64_t V, int64_t F, Layout& L) {
+  const size_t n = 3 * (size_t)F;
+  L.rows = 0;
+  L.table = L.rows + align_up(sizeof(float) * 9 * (size_t)F, kAlign);
+  L.keys_in = L.table + align_up(sizeof(int32_t) * ((size_t)V + 1 + n), kAlign);
+  L.keys_out = L.keys_in + align_up(sizeof(uint32_t) * n, kAlign);
+  L.ids_in = L.keys_out + align_up(sizeof(uint32_t) * n, kAlign);
+  L.cub = L.ids_in + align_up(sizeof(int32_t) * n, kAlign);
+  L.cub_bytes = 0;
+  if (n > 0 && cub::DeviceRadixSort::SortPairs(nullptr, L.cub_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                               (const int32_t*)nullptr, (int32_t*)nullptr, (int)n, 0,
+                                               key_bits(V)) != cudaSuccess)
+    return false;
+  L.total = L.cub + align_up(L.cub_bytes, kAlign);
+  return true;
+}
+
+int check_sizes(const char* op, int64_t V, int64_t F) {
+  if (V < 0 || F < 0) return fail(B200R_ERR_INVALID_ARGUMENT, std::string(op) + ": negative size");
+  if (V >= ((int64_t)1 << 31) - 1)
+    return fail(B200R_ERR_INVALID_ARGUMENT, std::string(op) + ": at most 2^31 - 2 vertices");
+  if (3 * F >= ((int64_t)1 << 31))
+    return fail(B200R_ERR_INVALID_ARGUMENT, std::string(op) + ": at most (2^31 - 1) / 3 faces (3F < 2^31 corners)");
+  return B200R_OK;
+}
+
+int checked_layout(const char* op, int64_t V, int64_t F, size_t workspace_bytes, const void* workspace, Layout& L) {
+  if (!layout(V, F, L)) {
+    cudaGetLastError();
+    return fail(B200R_ERR_CUDA, std::string(op) + ": cub could not size the sort's temporary storage");
+  }
+  if (workspace == nullptr || workspace_bytes < L.total)
+    return fail(B200R_ERR_INVALID_ARGUMENT, std::string(op) + ": workspace smaller than b200r_normals_workspace_bytes");
+  return B200R_OK;
+}
+
+dim3 grid_for(int64_t n) { return dim3((unsigned)cap_grid_stride_blocks((n + kThreads - 1) / kThreads)); }
+
+// Builds the table (offsets[V + 1], then the 3F corner ids in run order) at `table`.
+int build_table(const int64_t* faces, int64_t V, int64_t F, char* ws, const Layout& L, int32_t* table,
+                cudaStream_t stream) {
+  const int64_t n = 3 * F;
+  int32_t* offsets = table;
+  int32_t* corners = table + V + 1;
+  uint32_t* keys_in = reinterpret_cast<uint32_t*>(ws + L.keys_in);
+  uint32_t* keys_out = reinterpret_cast<uint32_t*>(ws + L.keys_out);
+  int32_t* ids_in = reinterpret_cast<int32_t*>(ws + L.ids_in);
+  if (n > 0) {
+    corner_keys_kernel<<<grid_for(F), kThreads, 0, stream>>>(faces, F, V, keys_in, ids_in);
+    B200R_LAUNCHED("corner_keys_kernel");
+    size_t cub_bytes = L.cub_bytes;
+    B200R_CUDA_OK(cub::DeviceRadixSort::SortPairs(ws + L.cub, cub_bytes, keys_in, keys_out, ids_in, corners, (int)n, 0,
+                                                  key_bits(V), stream));
+  }
+  run_offsets_kernel<<<grid_for(n + 1), kThreads, 0, stream>>>(keys_out, n, V, offsets);
+  B200R_LAUNCHED("run_offsets_kernel");
+  return B200R_OK;
+}
+
+}  // namespace
+}  // namespace b200r
+
+using namespace b200r;
+
+extern "C" size_t b200r_normals_workspace_bytes(int64_t V, int64_t F) {
+  if (V < 0 || F < 0) return 0;
+  Layout L;
+  if (!layout(V, F, L)) {
+    cudaGetLastError();
+    return 0;
+  }
+  return L.total;
+}
+
+extern "C" int b200r_verts_normals_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F,
+                                           void* workspace, size_t workspace_bytes, int32_t* table, float* sums,
+                                           float* normals, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int rc = check_sizes("verts_normals_forward", V, F);
+  if (rc != B200R_OK) return rc;
+  if (V == 0) return B200R_OK;
+  Layout L;
+  rc = checked_layout("verts_normals_forward", V, F, workspace_bytes, workspace, L);
+  if (rc != B200R_OK) return rc;
+  char* ws = static_cast<char*>(workspace);
+  float* rows = reinterpret_cast<float*>(ws + L.rows);
+  rc = build_table(faces, V, F, ws, L, table, stream);
+  if (rc != B200R_OK) return rc;
+  if (F > 0) {
+    face_normal_rows_kernel<<<grid_for(F), kThreads, 0, stream>>>(verts, faces, V, F, rows);
+    B200R_LAUNCHED("face_normal_rows_kernel");
+  }
+  segmented_sum_kernel<RowOf::kFace, Epilogue::kNormalize>
+      <<<grid_for(V), kThreads, 0, stream>>>(table, table + V + 1, V, F, rows, sums, normals);
+  B200R_LAUNCHED("segmented_sum_kernel");
+  return B200R_OK;
+}
+
+extern "C" int b200r_verts_normals_backward(const float* grad_normals, const float* verts, int64_t V,
+                                            const int64_t* faces, int64_t F, const int32_t* table, const float* sums,
+                                            void* workspace, size_t workspace_bytes, float* grad_verts,
+                                            void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int rc = check_sizes("verts_normals_backward", V, F);
+  if (rc != B200R_OK) return rc;
+  if (V == 0) return B200R_OK;
+  Layout L;
+  rc = checked_layout("verts_normals_backward", V, F, workspace_bytes, workspace, L);
+  if (rc != B200R_OK) return rc;
+  char* ws = static_cast<char*>(workspace);
+  float* rows = reinterpret_cast<float*>(ws + L.rows);
+  float* grad_sums = grad_verts;  // read by the rows kernel before the segmented sum overwrites it
+  normalize_backward_kernel<<<grid_for(V), kThreads, 0, stream>>>(grad_normals, sums, V, grad_sums);
+  B200R_LAUNCHED("normalize_backward_kernel");
+  if (F > 0) {
+    cross_backward_rows_kernel<<<grid_for(F), kThreads, 0, stream>>>(verts, faces, V, F, grad_sums, rows);
+    B200R_LAUNCHED("cross_backward_rows_kernel");
+  }
+  segmented_sum_kernel<RowOf::kCorner, Epilogue::kSum>
+      <<<grid_for(V), kThreads, 0, stream>>>(table, table + V + 1, V, F, rows, nullptr, grad_verts);
+  B200R_LAUNCHED("segmented_sum_kernel");
+  return B200R_OK;
+}
+
+extern "C" int b200r_face_areas_normals_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F,
+                                                float* areas, float* normals, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int rc = check_sizes("face_areas_normals_forward", V, F);
+  if (rc != B200R_OK) return rc;
+  if (F == 0) return B200R_OK;
+  face_areas_normals_forward_kernel<<<grid_for(F), kThreads, 0, stream>>>(verts, faces, V, F, areas, normals);
+  B200R_LAUNCHED("face_areas_normals_forward_kernel");
+  return B200R_OK;
+}
+
+extern "C" int b200r_face_areas_normals_backward(const float* grad_areas, const float* grad_normals,
+                                                 const float* verts, int64_t V, const int64_t* faces, int64_t F,
+                                                 void* workspace, size_t workspace_bytes, float* grad_verts,
+                                                 void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int rc = check_sizes("face_areas_normals_backward", V, F);
+  if (rc != B200R_OK) return rc;
+  if (V == 0) return B200R_OK;
+  Layout L;
+  rc = checked_layout("face_areas_normals_backward", V, F, workspace_bytes, workspace, L);
+  if (rc != B200R_OK) return rc;
+  char* ws = static_cast<char*>(workspace);
+  float* rows = reinterpret_cast<float*>(ws + L.rows);
+  int32_t* table = reinterpret_cast<int32_t*>(ws + L.table);
+  rc = build_table(faces, V, F, ws, L, table, stream);
+  if (rc != B200R_OK) return rc;
+  if (F > 0) {
+    face_areas_normals_backward_rows_kernel<<<grid_for(F), kThreads, 0, stream>>>(grad_areas, grad_normals, verts,
+                                                                                  faces, V, F, rows);
+    B200R_LAUNCHED("face_areas_normals_backward_rows_kernel");
+  }
+  segmented_sum_kernel<RowOf::kCorner, Epilogue::kSum>
+      <<<grid_for(V), kThreads, 0, stream>>>(table, table + V + 1, V, F, rows, nullptr, grad_verts);
+  B200R_LAUNCHED("segmented_sum_kernel");
+  return B200R_OK;
+}

@@ -65,6 +65,19 @@ perspective cameras:
 It replaces the two names in that module by functions that send float32 CUDA face_verts (and the Fragments of such a
 call) to `pytorch3d_b200.clip`'s fused pair, returning the reference's own `ClippedFaces`; everything else (CPU
 tensors, other dtypes) goes to the originals.
+
+`install_normals()` (separate again) serves the mesh normals that every lit shader, `sample_points_from_meshes` and
+the face-area users read:
+    pytorch3d/ops/mesh_face_areas_normals.py   from pytorch3d import _C   (face_areas_normals_forward/_backward)
+    pytorch3d/structures/meshes.py             Meshes._compute_vertex_normals (pure torch: a gather, torch.cross,
+                                               three index_add calls, F.normalize)
+It proxies `_C` of the first module for the two face ops: float32 CUDA verts with int64 CUDA faces on one device go to
+`pytorch3d_b200._C`, everything else (CPU tensors, float64 verts) to the original.  So `faces_normals_packed()`,
+`faces_areas_packed()`, HardFlatShader and `sample_points_from_meshes` run the new kernels.  It replaces the method
+`_compute_vertex_normals` on the class `Meshes`, as `install_textures()` does, keeping its `refresh` and caching
+semantics (including the `refresh=True` recomputation of `offset_verts_`): a non-empty mesh whose `verts_packed()` is
+float32 CUDA and `faces_packed()` int64 CUDA on the same device goes to `pytorch3d_b200.normals.verts_normals`;
+everything else, empty meshes included (the original stores an int64 (N, 3) zero tensor), to the original method.
 """
 import importlib
 import types
@@ -89,29 +102,42 @@ _SHADING_FUNCTIONS = ("phong_shading", "_phong_shading_with_pixels", "flat_shadi
 _TEXTURES_MODULE = "pytorch3d.renderer.mesh.textures"
 _CLIP_MODULE = "pytorch3d.renderer.mesh.rasterize_meshes"
 _CLIP_FUNCTIONS = ("clip_faces", "convert_clipped_rasterization_to_original_faces")
+_NORMALS_MODULE = "pytorch3d.ops.mesh_face_areas_normals"
+_NORMALS_OPS = ("face_areas_normals_forward", "face_areas_normals_backward")
+_MESHES_MODULE = "pytorch3d.structures.meshes"
 _saved = {}
-# (module name, attribute) -> original (install_blending, install_splatter, install_shading, install_gouraud and
-# install_clipping)
+# (module name, attribute) -> original (install_blending, install_splatter, install_shading, install_gouraud,
+# install_clipping and install_normals)
 _saved_blend = {}
-_saved_methods = {}  # (module name, class name, method name) -> original (install_textures, install_texture_atlas)
+# (module name, class name, method name) -> original (install_textures, install_texture_atlas, install_normals)
+_saved_methods = {}
+
+
+def _first_is_cuda(name, args):
+    first = args[0] if args else None
+    return first is None or getattr(first, "is_cuda", False)
 
 
 class _Proxy(types.ModuleType):
-    def __init__(self, original, ops=_OPS):
+    """`ops` are served by `pytorch3d_b200._C` when `fused(name, args)` holds (by default: the first argument is a CUDA
+    tensor) and by the original module otherwise; every other name is the original's."""
+
+    def __init__(self, original, ops=_OPS, fused=_first_is_cuda):
         super().__init__("pytorch3d_b200._C_proxy")
         self.__dict__["_original"] = original
         self.__dict__["_ops"] = ops
+        self.__dict__["_fused"] = fused
 
     def __getattr__(self, name):
         original = self.__dict__["_original"]
         if name in self.__dict__["_ops"]:
             ours = getattr(_b200_C, name)
             theirs = getattr(original, name, None)
+            fused = self.__dict__["_fused"]
 
             def dispatch(*args, **kwargs):
-                first = args[0] if args else None
-                if theirs is not None and first is not None and not getattr(first, "is_cuda", False):
-                    return theirs(*args, **kwargs)  # CPU tensors keep the reference's CPU path
+                if theirs is not None and not fused(name, args):
+                    return theirs(*args, **kwargs)  # e.g. CPU tensors keep the reference's CPU path
                 return ours(*args, **kwargs)
 
             return dispatch
@@ -469,9 +495,64 @@ def install_clipping():
     return [_CLIP_MODULE]
 
 
+def _mesh_fused(verts, faces):
+    """Whether the fused normal ops take these packed tensors: float32 CUDA verts (V, 3) and int64 CUDA faces (F, 3) on
+    one device, within the kernels' size limits."""
+    if not (getattr(verts, "is_cuda", False) and getattr(faces, "is_cuda", False) and verts.device == faces.device):
+        return False
+    if verts.dtype != torch.float32 or faces.dtype != torch.int64:
+        return False
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        return False
+    return verts.shape[0] < (1 << 31) - 1 and 3 * faces.shape[0] < (1 << 31)
+
+
+def _face_normals_fused(name, args):
+    """The proxied face ops: verts is argument 0 of the forward and 2 of the backward."""
+    verts_at = 0 if name == "face_areas_normals_forward" else 2
+    if len(args) <= verts_at + 1:
+        return False
+    return _mesh_fused(args[verts_at], args[verts_at + 1])
+
+
+def _vertex_normals_dispatch(original):
+    from . import normals as ours
+
+    def _compute_vertex_normals(self, refresh: bool = False):
+        if not (refresh or any(v is None for v in [self._verts_normals_packed])):
+            return
+        if not self.isempty():
+            verts, faces = self.verts_packed(), self.faces_packed()
+            if _mesh_fused(verts, faces):
+                self._verts_normals_packed = ours.verts_normals(verts, faces)
+                return
+        return original(self, refresh=refresh)
+
+    _compute_vertex_normals.__qualname__ = "Meshes._compute_vertex_normals"
+    _compute_vertex_normals.__doc__ = original.__doc__
+    return _compute_vertex_normals
+
+
+def install_normals():
+    """Patch PyTorch3D's mesh normals (must be importable): `_C` in pytorch3d.ops.mesh_face_areas_normals for the two
+    face ops, and the method `_compute_vertex_normals` of the class `Meshes` in pytorch3d.structures.meshes.  Returns
+    the list of patched module names."""
+    mod = importlib.import_module(_NORMALS_MODULE)
+    if (_NORMALS_MODULE, "_C") not in _saved_blend:
+        _saved_blend[(_NORMALS_MODULE, "_C")] = mod._C
+        mod._C = _Proxy(mod._C, _NORMALS_OPS, _face_normals_fused)
+    m = importlib.import_module(_MESHES_MODULE)
+    key = (_MESHES_MODULE, "Meshes", "_compute_vertex_normals")
+    if key not in _saved_methods:
+        cls = m.Meshes
+        _saved_methods[key] = cls.__dict__["_compute_vertex_normals"]
+        cls._compute_vertex_normals = _vertex_normals_dispatch(cls.__dict__["_compute_vertex_normals"])
+    return [_NORMALS_MODULE, _MESHES_MODULE]
+
+
 def uninstall():
     """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_gouraud()`,
-    `install_textures()`, `install_texture_atlas()` and `install_clipping()`."""
+    `install_textures()`, `install_texture_atlas()`, `install_clipping()` and `install_normals()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
