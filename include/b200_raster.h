@@ -454,6 +454,62 @@ int b200r_verts_normals_backward(const float* grad_normals, const float* verts, 
                                  size_t workspace_bytes, float* grad_verts, void* stream);
 
 /*
+ * Mesh regularisers (DESIGN.md section 18): what pytorch3d/loss/mesh_edge_loss.py, mesh_laplacian_smoothing.py and
+ * mesh_normal_consistency.py compute, as a float32 scalar `loss` (a device pointer), and its gradient to the verts.
+ *  verts float32 (V,3) and faces int64 (F,3), contiguous, read in place (64-bit offsets); V < 2^31 - 1 and 6F < 2^31,
+ *  larger sizes return B200R_ERR_INVALID_ARGUMENT.  mesh_first_vert, mesh_num_verts int64 (N,) device arrays, as
+ *  b200r_gouraud_* takes them: mesh m owns vertices [first[m], first[m] + num[m]), the ranges ascending and covering
+ *  every vertex; N >= 1 (the loss is divided by N, empty meshes included).  A face index outside [0, V) belongs to no
+ *  edge and no vertex.  All entry points are asynchronous, use no float atomics and are deterministic.
+ *  Edges are the distinct (min, max) vertex pairs of the face-edges in ascending order, as Meshes.edges_packed();
+ *  self-loops included.
+ * edge loss: sum over edges of (|v0 - v1| - target_length)^2 / (edges of the mesh), over N.
+ * Laplacian smoothing: sum over vertices of |y_v| / (vertices of the mesh), over N, with y = L v for method
+ *  B200R_LAPLACIAN_UNIFORM, the cotangent rows of cot_laplacian() for _COT and _COTCURV; L and its weights are
+ *  constants of the backward.  Another method returns B200R_ERR_INVALID_ARGUMENT.
+ * normal consistency: over every pair of face-edges on one edge, 1 - cos(n_a, -n_b), n = sum_k (v1 - v0) x (f_k - v0),
+ *  weighted by 1 / (pairs of the mesh), over N.  With no pair at all the loss is 0 and its gradient 0.
+ * workspace: b200r_regularizers_workspace_bytes(V, F, N) bytes, a function of the shapes only (0 when there is no
+ *  device to size the sorts for).  The forward leaves its tables there; the backward takes the same buffer, as the
+ *  forward of the same loss (and method) on the same faces left it, and the same arguments, and does not sort again.
+ *  grad_loss is a float32 device scalar; grad_verts (V,3) is fully written.
+ * mesh_edge_table: the edge table alone, for tests: edges int64 (3F,2) (the first E rows written), face_to_edge int64
+ *  (F,3) (faces_packed_to_edges_packed; -1 for a face-edge with a vertex out of range), num_edges_per_mesh int64 (N,)
+ *  and E int64 (1,), all device arrays.
+ */
+#define B200R_LAPLACIAN_UNIFORM 0
+#define B200R_LAPLACIAN_COT 1
+#define B200R_LAPLACIAN_COTCURV 2
+size_t b200r_regularizers_workspace_bytes(int64_t V, int64_t F, int32_t N);
+int b200r_mesh_edge_table(const int64_t* faces, int64_t V, int64_t F, const int64_t* mesh_first_vert,
+                          const int64_t* mesh_num_verts, int32_t N, void* workspace, size_t workspace_bytes,
+                          int64_t* edges, int64_t* face_to_edge, int64_t* num_edges_per_mesh, int64_t* num_edges,
+                          void* stream);
+int b200r_mesh_edge_loss_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F,
+                                 const int64_t* mesh_first_vert, const int64_t* mesh_num_verts, int32_t N,
+                                 float target_length, void* workspace, size_t workspace_bytes, float* loss,
+                                 void* stream);
+int b200r_mesh_edge_loss_backward(const float* grad_loss, const float* verts, int64_t V, const int64_t* faces,
+                                  int64_t F, const int64_t* mesh_first_vert, const int64_t* mesh_num_verts, int32_t N,
+                                  float target_length, void* workspace, size_t workspace_bytes, float* grad_verts,
+                                  void* stream);
+int b200r_mesh_laplacian_smoothing_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F,
+                                           const int64_t* mesh_first_vert, const int64_t* mesh_num_verts, int32_t N,
+                                           int32_t method, void* workspace, size_t workspace_bytes, float* loss,
+                                           void* stream);
+int b200r_mesh_laplacian_smoothing_backward(const float* grad_loss, const float* verts, int64_t V,
+                                            const int64_t* faces, int64_t F, const int64_t* mesh_first_vert,
+                                            const int64_t* mesh_num_verts, int32_t N, int32_t method, void* workspace,
+                                            size_t workspace_bytes, float* grad_verts, void* stream);
+int b200r_mesh_normal_consistency_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F,
+                                          const int64_t* mesh_first_vert, const int64_t* mesh_num_verts, int32_t N,
+                                          void* workspace, size_t workspace_bytes, float* loss, void* stream);
+int b200r_mesh_normal_consistency_backward(const float* grad_loss, const float* verts, int64_t V,
+                                           const int64_t* faces, int64_t F, const int64_t* mesh_first_vert,
+                                           const int64_t* mesh_num_verts, int32_t N, void* workspace,
+                                           size_t workspace_bytes, float* grad_verts, void* stream);
+
+/*
  * Fused frustum culling and z-clipping (additional entry points, no counterpart in pytorch3d._C): what
  * pytorch3d/renderer/mesh/clip.py clip_faces and convert_clipped_rasterization_to_original_faces compute, with the
  * reference's output layout (DESIGN.md section 14).  All entry points are asynchronous.

@@ -1076,6 +1076,188 @@ def verts_normals_backward(grad_normals: torch.Tensor, verts: torch.Tensor, face
     return grad_verts
 
 
+LAPLACIAN_METHODS = {"uniform": 0, "cot": 1, "cotcurv": 2}  # B200R_LAPLACIAN_*
+
+
+def _check_regularizer_inputs(op, verts, faces, mesh_first_vert, mesh_num_verts):
+    """(V, F, N, device) of float32 verts (V, 3), int64 faces (F, 3) and the int64 (N,) per-mesh vertex ranges, all on
+    one CUDA device, N >= 1; raises RuntimeError otherwise and for sizes past the kernels' limits (V < 2^31 - 1,
+    6F < 2^31)."""
+    dev = _require_cuda(("verts", verts), ("faces", faces), ("mesh_first_vert", mesh_first_vert),
+                        ("mesh_num_verts", mesh_num_verts))
+    if verts.dtype != torch.float32:
+        raise RuntimeError("%s: expected scalar type Float for verts but found %s" % (op, verts.dtype))
+    if faces.dtype != torch.int64:
+        raise RuntimeError("%s: expected scalar type Long for faces but found %s" % (op, faces.dtype))
+    if verts.dim() != 2 or verts.shape[1] != 3:
+        raise RuntimeError("%s: verts must be (V, 3), got %s" % (op, tuple(verts.shape)))
+    if faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError("%s: faces must be (F, 3), got %s" % (op, tuple(faces.shape)))
+    N = int(mesh_first_vert.shape[0]) if mesh_first_vert.dim() == 1 else -1
+    for name, t in (("mesh_first_vert", mesh_first_vert), ("mesh_num_verts", mesh_num_verts)):
+        if t.dtype != torch.int64 or t.dim() != 1 or t.shape[0] != N or N < 1:
+            raise RuntimeError("%s: %s must be an int64 (N,) tensor with N >= 1 like mesh_first_vert, got %s %s"
+                               % (op, name, t.dtype, tuple(t.shape)))
+    V, F = int(verts.shape[0]), int(faces.shape[0])
+    if V >= (1 << 31) - 1 or 6 * F >= (1 << 31) or N >= (1 << 31):
+        raise RuntimeError("%s: at most 2^31 - 2 vertices and (2^31 - 1) / 6 faces, got V = %d, F = %d" % (op, V, F))
+    return V, F, N, dev
+
+
+def _regularizer_workspace(lib, V, F, N, dev):
+    ws_bytes = int(lib.b200r_regularizers_workspace_bytes(V, F, N))
+    return torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None, ws_bytes
+
+
+def _check_workspace(workspace, ws_bytes, dev):
+    if workspace is None and ws_bytes == 0:
+        return
+    if (workspace is None or not workspace.is_cuda or workspace.device != dev or workspace.dtype != torch.uint8
+            or workspace.numel() < ws_bytes or not workspace.is_contiguous()):
+        raise RuntimeError("workspace must be the uint8 workspace of the matching forward on %s" % dev)
+
+
+def _check_grad_loss(grad_loss, dev):
+    g = _check_grad("grad_loss", grad_loss.reshape(()) if grad_loss.numel() == 1 else grad_loss, (), dev)
+    return g
+
+
+def mesh_edge_table(faces: torch.Tensor, V: int, mesh_first_vert: torch.Tensor, mesh_num_verts: torch.Tensor):
+    """The edge table of the regularisers, for tests: faces (F,3) i64 with vertices in [0, V), the per-mesh vertex
+    ranges -> (edges (E,2) i64, face_to_edge (F,3) i64, num_edges_per_mesh (N,) i64), PyTorch3D's edges_packed(),
+    faces_packed_to_edges_packed() and num_edges_per_mesh().  Reads E on the host."""
+    verts = torch.empty((int(V), 3), dtype=torch.float32, device=faces.device) if faces.is_cuda else \
+        torch.empty((int(V), 3))
+    V, F, N, dev = _check_regularizer_inputs("mesh_edge_table", verts, faces, mesh_first_vert, mesh_num_verts)
+    lib = _lib.load()
+    f, first, num = faces.contiguous(), mesh_first_vert.contiguous(), mesh_num_verts.contiguous()
+    with torch.cuda.device(dev):
+        edges = torch.empty((3 * F, 2), dtype=torch.int64, device=dev)
+        face_to_edge = torch.empty((F, 3), dtype=torch.int64, device=dev)
+        counts = torch.empty((N,), dtype=torch.int64, device=dev)
+        E = torch.empty((1,), dtype=torch.int64, device=dev)
+        ws, ws_bytes = _regularizer_workspace(lib, V, F, N, dev)
+        _lib.check(lib.b200r_mesh_edge_table(_ptr(f), V, F, _ptr(first), _ptr(num), N, _ptr(ws), ws_bytes,
+                                             _ptr(edges), _ptr(face_to_edge), _ptr(counts), _ptr(E),
+                                             _stream_ptr(dev)))
+    return edges[:int(E.item())], face_to_edge, counts
+
+
+def mesh_edge_loss_forward(verts, faces, mesh_first_vert, mesh_num_verts, target_length: float):
+    """Fused pytorch3d.loss.mesh_edge_loss (DESIGN.md section 18) -> (loss () f32, workspace): the workspace holds the
+    tables `mesh_edge_loss_backward` reads."""
+    V, F, N, dev = _check_regularizer_inputs("mesh_edge_loss_forward", verts, faces, mesh_first_vert, mesh_num_verts)
+    lib = _lib.load()
+    v, f = verts.contiguous(), faces.contiguous()
+    with torch.cuda.device(dev):
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        ws, ws_bytes = _regularizer_workspace(lib, V, F, N, dev)
+        _lib.check(lib.b200r_mesh_edge_loss_forward(_ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()),
+                                                    _ptr(mesh_num_verts.contiguous()), N, float(target_length),
+                                                    _ptr(ws), ws_bytes, loss.data_ptr(), _stream_ptr(dev)))
+    return loss, ws
+
+
+def mesh_edge_loss_backward(grad_loss, verts, faces, mesh_first_vert, mesh_num_verts, target_length: float,
+                            workspace):
+    """Backward of `mesh_edge_loss_forward` -> grad_verts (V,3) f32, from the forward's workspace (no sort).
+    Deterministic, no atomics; grad_loss stays on the device."""
+    V, F, N, dev = _check_regularizer_inputs("mesh_edge_loss_backward", verts, faces, mesh_first_vert, mesh_num_verts)
+    g = _check_grad_loss(grad_loss, dev)
+    lib = _lib.load()
+    ws_bytes = int(lib.b200r_regularizers_workspace_bytes(V, F, N))
+    _check_workspace(workspace, ws_bytes, dev)
+    v, f = verts.contiguous(), faces.contiguous()
+    with torch.cuda.device(dev):
+        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        _lib.check(lib.b200r_mesh_edge_loss_backward(g.data_ptr(), _ptr(v), V, _ptr(f), F,
+                                                     _ptr(mesh_first_vert.contiguous()),
+                                                     _ptr(mesh_num_verts.contiguous()), N, float(target_length),
+                                                     _ptr(workspace), ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
+    return grad_verts
+
+
+def _laplacian_method(method):
+    if method not in LAPLACIAN_METHODS:
+        raise ValueError("Method should be one of {uniform, cot, cotcurv}")
+    return LAPLACIAN_METHODS[method]
+
+
+def mesh_laplacian_smoothing_forward(verts, faces, mesh_first_vert, mesh_num_verts, method: str):
+    """Fused pytorch3d.loss.mesh_laplacian_smoothing for method "uniform", "cot" or "cotcurv" (DESIGN.md section 18)
+    -> (loss () f32, workspace)."""
+    m = _laplacian_method(method)
+    V, F, N, dev = _check_regularizer_inputs("mesh_laplacian_smoothing_forward", verts, faces, mesh_first_vert,
+                                             mesh_num_verts)
+    lib = _lib.load()
+    v, f = verts.contiguous(), faces.contiguous()
+    with torch.cuda.device(dev):
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        ws, ws_bytes = _regularizer_workspace(lib, V, F, N, dev)
+        _lib.check(lib.b200r_mesh_laplacian_smoothing_forward(
+            _ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()), _ptr(mesh_num_verts.contiguous()), N, m,
+            _ptr(ws), ws_bytes, loss.data_ptr(), _stream_ptr(dev)))
+    return loss, ws
+
+
+def mesh_laplacian_smoothing_backward(grad_loss, verts, faces, mesh_first_vert, mesh_num_verts, method: str,
+                                      workspace):
+    """Backward of `mesh_laplacian_smoothing_forward` -> grad_verts (V,3) f32, with L and its weights constant (no
+    sort).  Deterministic, no atomics."""
+    m = _laplacian_method(method)
+    V, F, N, dev = _check_regularizer_inputs("mesh_laplacian_smoothing_backward", verts, faces, mesh_first_vert,
+                                             mesh_num_verts)
+    g = _check_grad_loss(grad_loss, dev)
+    lib = _lib.load()
+    ws_bytes = int(lib.b200r_regularizers_workspace_bytes(V, F, N))
+    _check_workspace(workspace, ws_bytes, dev)
+    v, f = verts.contiguous(), faces.contiguous()
+    with torch.cuda.device(dev):
+        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        _lib.check(lib.b200r_mesh_laplacian_smoothing_backward(
+            g.data_ptr(), _ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()),
+            _ptr(mesh_num_verts.contiguous()), N, m, _ptr(workspace), ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
+    return grad_verts
+
+
+def mesh_normal_consistency_forward(verts, faces, mesh_first_vert, mesh_num_verts):
+    """Fused pytorch3d.loss.mesh_normal_consistency (DESIGN.md section 18) -> (loss () f32, workspace).  The face pairs
+    are enumerated on the device: nothing reads the edge counts on the host."""
+    V, F, N, dev = _check_regularizer_inputs("mesh_normal_consistency_forward", verts, faces, mesh_first_vert,
+                                             mesh_num_verts)
+    lib = _lib.load()
+    v, f = verts.contiguous(), faces.contiguous()
+    with torch.cuda.device(dev):
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        ws, ws_bytes = _regularizer_workspace(lib, V, F, N, dev)
+        _lib.check(lib.b200r_mesh_normal_consistency_forward(
+            _ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()), _ptr(mesh_num_verts.contiguous()), N,
+            _ptr(ws), ws_bytes, loss.data_ptr(), _stream_ptr(dev)))
+    return loss, ws
+
+
+def mesh_normal_consistency_backward(grad_loss, verts, faces, mesh_first_vert, mesh_num_verts, workspace):
+    """Backward of `mesh_normal_consistency_forward` -> grad_verts (V,3) f32 (no sort, no scatter).  Deterministic,
+    no atomics."""
+    V, F, N, dev = _check_regularizer_inputs("mesh_normal_consistency_backward", verts, faces, mesh_first_vert,
+                                             mesh_num_verts)
+    g = _check_grad_loss(grad_loss, dev)
+    lib = _lib.load()
+    ws_bytes = int(lib.b200r_regularizers_workspace_bytes(V, F, N))
+    _check_workspace(workspace, ws_bytes, dev)
+    v, f = verts.contiguous(), faces.contiguous()
+    with torch.cuda.device(dev):
+        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        _lib.check(lib.b200r_mesh_normal_consistency_backward(
+            g.data_ptr(), _ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()),
+            _ptr(mesh_num_verts.contiguous()), N, _ptr(workspace), ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
+    return grad_verts
+
+
+# the name the test hook is known by
+_mesh_edge_table = mesh_edge_table
+
+
 def _clip_frustum_args(frustum):
     """(planes (6,) float32 host array, cull_mask, has_z_clip, z_clip, perspective_correct) of a ClipFrustum-like
     object for the b200r_clip_* entry points."""

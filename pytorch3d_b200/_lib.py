@@ -103,6 +103,18 @@ SIGNATURES = {
     "b200r_face_areas_normals_backward": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
     "b200r_verts_normals_forward": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp, _vp, _vp]),
     "b200r_verts_normals_backward": (ctypes.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "b200r_regularizers_workspace_bytes": (_sz, [_i64, _i64, _i32]),
+    "b200r_mesh_edge_table": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _i32, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
+    "b200r_mesh_edge_loss_forward": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i32, _f32, _vp, _sz, _vp, _vp]),
+    "b200r_mesh_edge_loss_backward": (
+        ctypes.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _i32, _f32, _vp, _sz, _vp, _vp]),
+    "b200r_mesh_laplacian_smoothing_forward": (
+        ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i32, _i32, _vp, _sz, _vp, _vp]),
+    "b200r_mesh_laplacian_smoothing_backward": (
+        ctypes.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _i32, _i32, _vp, _sz, _vp, _vp]),
+    "b200r_mesh_normal_consistency_forward": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i32, _vp, _sz, _vp, _vp]),
+    "b200r_mesh_normal_consistency_backward": (
+        ctypes.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _i32, _vp, _sz, _vp, _vp]),
     "b200r_clip_faces_workspace_words": (_i64, [_i64]),
     "b200r_clip_faces_count": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i32, _i32, _f64, _vp, _vp]),
     "b200r_clip_faces_fill": (

@@ -1,12 +1,12 @@
 // Mesh normals: vertex normals and face areas / normals, forward and deterministic backward (DESIGN.md section 17).
 //
-// Both ops rest on one structure, the vertex -> corner table.  Corner j of face f has the id c = j * F + f and the key
-// faces[f, j]; a stable radix sort of the 3F (key, id) pairs over ceil(log2(V + 1)) key bits, and an offset array of
-// V + 1 entries, give every vertex the run of its corners in (j, f) order.  That is the order in which the three
-// serial index_add calls of pytorch3d/structures/meshes.py Meshes._compute_vertex_normals accumulate on the CPU.  Every
-// per-vertex sum is one thread walking its run from +0 with __fadd_rn (segmented_sum_kernel, shared by both ops), so
-// there are no float atomics and the results do not depend on scheduling.  Nothing synchronises the host, and the
-// workspace depends only on (V, F).
+// Both ops rest on one structure, the vertex -> corner table (mesh_tables.cuh).  Corner j of face f has the id
+// c = j * F + f and the key faces[f, j]; a stable radix sort of the 3F (key, id) pairs over ceil(log2(V + 1)) key bits,
+// and an offset array of V + 1 entries, give every vertex the run of its corners in (j, f) order.  That is the order in
+// which the three serial index_add calls of pytorch3d/structures/meshes.py Meshes._compute_vertex_normals accumulate on
+// the CPU.  Every per-vertex sum is one thread walking its run from +0 with __fadd_rn (segmented_sum_kernel, shared by
+// both ops), so there are no float atomics and the results do not depend on scheduling.  Nothing synchronises the
+// host, and the workspace depends only on (V, F).
 //
 // Vertex normals (Meshes._compute_vertex_normals, restated with explicit rounding):
 //   n_f = (v2 - v1) x (v0 - v1), each component fma(a_i, b_j, -rn(a_j * b_i)) with a = v2 - v1, b = v0 - v1
@@ -20,121 +20,15 @@
 // 1e-6, norm / 2.0), so the results are bit-identical.  The backward writes the reference's nine per-corner expressions,
 // in its arithmetic, to an (F, 3, 3) workspace, and sums them per vertex over a table built in the same call instead of
 // adding them with float atomics.
-#include <cub/device/device_radix_sort.cuh>
-
-#include "common.cuh"
+#include "mesh_tables.cuh"
 
 namespace b200r {
 namespace {
 
-constexpr int kThreads = 256;
-constexpr float kNormalizeEps = 1e-6f;  // F.normalize(..., eps=1e-6) in Meshes._compute_vertex_normals
 constexpr size_t kAlign = 256;
-
-// The three corners of face f.  A face index outside [0, V) (the reference does not check them either) gives NaN
-// corners instead of a read out of bounds.
-__device__ __forceinline__ void face_corners(const float* __restrict__ verts, const int64_t* __restrict__ faces,
-                                             int64_t V, int64_t f, float3 p[3]) {
-#pragma unroll
-  for (int j = 0; j < 3; ++j) {
-    const int64_t v = __ldg(faces + 3 * f + j);
-    if (v >= 0 && v < V) {
-      p[j] = make_float3(__ldg(verts + 3 * v + 0), __ldg(verts + 3 * v + 1), __ldg(verts + 3 * v + 2));
-    } else {
-      const float nan = __int_as_float(0x7fc00000);
-      p[j] = make_float3(nan, nan, nan);
-    }
-  }
-}
 
 __device__ __forceinline__ float3 sub_rn(float3 a, float3 b) {
   return make_float3(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z));
-}
-
-// a x b with each component fma(a_i, b_j, -rn(a_j * b_i)): torch.cross on float32 as compiled for the CPU, and autograd's
-// cross backward.
-__device__ __forceinline__ float3 cross_fma(float3 a, float3 b) {
-  return make_float3(__fmaf_rn(a.y, b.z, -__fmul_rn(a.z, b.y)), __fmaf_rn(a.z, b.x, -__fmul_rn(a.x, b.z)),
-                     __fmaf_rn(a.x, b.y, -__fmul_rn(a.y, b.x)));
-}
-
-// |s| as torch's 2-norm over dim 1 of a float32 (V, 3) tensor computes it.
-__device__ __forceinline__ float norm3(float3 s) {
-  return __fsqrt_rn(__fmaf_rn(s.z, s.z, __fmaf_rn(s.y, s.y, __fmul_rn(s.x, s.x))));
-}
-
-__device__ __forceinline__ float3 load3(const float* __restrict__ p, int64_t i) {
-  return make_float3(__ldg(p + 3 * i + 0), __ldg(p + 3 * i + 1), __ldg(p + 3 * i + 2));
-}
-
-__device__ __forceinline__ void store3(float* __restrict__ p, int64_t i, float3 v) {
-  p[3 * i + 0] = v.x;
-  p[3 * i + 1] = v.y;
-  p[3 * i + 2] = v.z;
-}
-
-// ---- the vertex -> corner table ---------------------------------------------------------------------------------
-
-// (key, corner id) of every corner; a face index outside [0, V) gets the key V, which sorts after every vertex and
-// belongs to no run.
-__global__ void __launch_bounds__(kThreads)
-    corner_keys_kernel(const int64_t* __restrict__ faces, int64_t F, int64_t V, uint32_t* __restrict__ keys,
-                       int32_t* __restrict__ ids) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += stride) {
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const int64_t v = __ldg(faces + 3 * f + j);
-      const int64_t c = j * F + f;
-      keys[c] = (uint32_t)((v >= 0 && v < V) ? v : V);
-      ids[c] = (int32_t)c;
-    }
-  }
-}
-
-// offsets[v] = the first sorted position whose key is >= v, for v in [0, V]: position i writes the offsets of the
-// vertices after the previous key up to its own (the end, n, stands for the key V).
-__global__ void __launch_bounds__(kThreads)
-    run_offsets_kernel(const uint32_t* __restrict__ keys, int64_t n, int64_t V, int32_t* __restrict__ offsets) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += stride) {
-    const int64_t prev = i > 0 ? (int64_t)keys[i - 1] : -1;
-    const int64_t cur = i < n ? (int64_t)keys[i] : V;
-    for (int64_t v = prev + 1; v <= cur; ++v) offsets[v] = (int32_t)i;
-  }
-}
-
-// ---- the one segmented sum --------------------------------------------------------------------------------------
-
-enum class RowOf { kFace, kCorner };   // rows[f] (F, 3) or rows[f * 3 + j] (F, 3, 3)
-enum class Epilogue { kSum, kNormalize };
-
-// Per vertex: the sum of its corners' rows in run order from +0.  kNormalize also stores the sum in `sums` and writes
-// sum / max(|sum|, 1e-6) to `out`.
-template <RowOf ROW, Epilogue EPI>
-__global__ void __launch_bounds__(kThreads)
-    segmented_sum_kernel(const int32_t* __restrict__ offsets, const int32_t* __restrict__ corners, int64_t V,
-                         int64_t F, const float* __restrict__ rows, float* __restrict__ sums,
-                         float* __restrict__ out) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < V; v += stride) {
-    const int32_t end = __ldg(offsets + v + 1);
-    float3 acc = make_float3(0.0f, 0.0f, 0.0f);
-    for (int32_t i = __ldg(offsets + v); i < end; ++i) {
-      const int64_t c = __ldg(corners + i);
-      const int64_t j = c >= 2 * F ? 2 : (c >= F ? 1 : 0);
-      const int64_t f = c - j * F;
-      const float3 r = load3(rows, ROW == RowOf::kFace ? f : f * 3 + j);
-      acc = make_float3(__fadd_rn(acc.x, r.x), __fadd_rn(acc.y, r.y), __fadd_rn(acc.z, r.z));
-    }
-    if (EPI == Epilogue::kNormalize) {
-      store3(sums, v, acc);
-      const float n = norm3(acc);
-      const float m = n < kNormalizeEps ? kNormalizeEps : n;  // clamp_min: NaN stays NaN
-      acc = make_float3(__fdiv_rn(acc.x, m), __fdiv_rn(acc.y, m), __fdiv_rn(acc.z, m));
-    }
-    store3(out, v, acc);
-  }
 }
 
 // ---- vertex normals -----------------------------------------------------------------------------------------------
@@ -283,13 +177,6 @@ __global__ void __launch_bounds__(kThreads)
 
 // ---- host side ----------------------------------------------------------------------------------------------------
 
-// ceil(log2(V + 1)): the key bits the sort looks at (the key V, for faces out of range, included).
-int key_bits(int64_t V) {
-  int bits = 1;
-  while (bits < 32 && (V >> bits) != 0) ++bits;
-  return bits;
-}
-
 // Workspace: rows (9F floats), a table (V + 1 + 3F ints), keys in / out and ids (3F each), then cub's temporary
 // storage.  Returns false when cub cannot size its storage (no device).
 struct Layout {
@@ -304,11 +191,7 @@ bool layout(int64_t V, int64_t F, Layout& L) {
   L.keys_out = L.keys_in + align_up(sizeof(uint32_t) * n, kAlign);
   L.ids_in = L.keys_out + align_up(sizeof(uint32_t) * n, kAlign);
   L.cub = L.ids_in + align_up(sizeof(int32_t) * n, kAlign);
-  L.cub_bytes = 0;
-  if (n > 0 && cub::DeviceRadixSort::SortPairs(nullptr, L.cub_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
-                                               (const int32_t*)nullptr, (int32_t*)nullptr, (int)n, 0,
-                                               key_bits(V)) != cudaSuccess)
-    return false;
+  if (!corner_sort_bytes(V, n, L.cub_bytes)) return false;
   L.total = L.cub + align_up(L.cub_bytes, kAlign);
   return true;
 }
@@ -332,27 +215,12 @@ int checked_layout(const char* op, int64_t V, int64_t F, size_t workspace_bytes,
   return B200R_OK;
 }
 
-dim3 grid_for(int64_t n) { return dim3((unsigned)cap_grid_stride_blocks((n + kThreads - 1) / kThreads)); }
-
 // Builds the table (offsets[V + 1], then the 3F corner ids in run order) at `table`.
 int build_table(const int64_t* faces, int64_t V, int64_t F, char* ws, const Layout& L, int32_t* table,
                 cudaStream_t stream) {
-  const int64_t n = 3 * F;
-  int32_t* offsets = table;
-  int32_t* corners = table + V + 1;
-  uint32_t* keys_in = reinterpret_cast<uint32_t*>(ws + L.keys_in);
-  uint32_t* keys_out = reinterpret_cast<uint32_t*>(ws + L.keys_out);
-  int32_t* ids_in = reinterpret_cast<int32_t*>(ws + L.ids_in);
-  if (n > 0) {
-    corner_keys_kernel<<<grid_for(F), kThreads, 0, stream>>>(faces, F, V, keys_in, ids_in);
-    B200R_LAUNCHED("corner_keys_kernel");
-    size_t cub_bytes = L.cub_bytes;
-    B200R_CUDA_OK(cub::DeviceRadixSort::SortPairs(ws + L.cub, cub_bytes, keys_in, keys_out, ids_in, corners, (int)n, 0,
-                                                  key_bits(V), stream));
-  }
-  run_offsets_kernel<<<grid_for(n + 1), kThreads, 0, stream>>>(keys_out, n, V, offsets);
-  B200R_LAUNCHED("run_offsets_kernel");
-  return B200R_OK;
+  return build_table(faces, V, F, reinterpret_cast<uint32_t*>(ws + L.keys_in),
+                     reinterpret_cast<uint32_t*>(ws + L.keys_out), reinterpret_cast<int32_t*>(ws + L.ids_in),
+                     ws + L.cub, L.cub_bytes, table, stream);
 }
 
 }  // namespace

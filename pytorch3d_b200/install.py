@@ -78,6 +78,16 @@ It proxies `_C` of the first module for the two face ops: float32 CUDA verts wit
 semantics (including the `refresh=True` recomputation of `offset_verts_`): a non-empty mesh whose `verts_packed()` is
 float32 CUDA and `faces_packed()` int64 CUDA on the same device goes to `pytorch3d_b200.normals.verts_normals`;
 everything else, empty meshes included (the original stores an int64 (N, 3) zero tensor), to the original method.
+
+`install_regularizers()` (separate again) serves the three shape priors of a mesh-fitting loop:
+    pytorch3d/loss/__init__.py                      from .mesh_edge_loss import mesh_edge_loss, ... (by name)
+    pytorch3d/loss/mesh_edge_loss.py                mesh_edge_loss (torch: edges_packed(), a gather, a norm)
+    pytorch3d/loss/mesh_laplacian_smoothing.py      mesh_laplacian_smoothing (sparse matrices, cuSPARSE)
+    pytorch3d/loss/mesh_normal_consistency.py       mesh_normal_consistency (a host copy, a CPU pair enumeration)
+It replaces the three names in `pytorch3d.loss` and in their defining modules by functions that send meshes whose
+`verts_packed()` is float32 CUDA and `faces_packed()` int64 CUDA on the same device, within the kernels' size limits
+(V < 2^31 - 1, 6F < 2^31), to `pytorch3d_b200.regularizers`; everything else (CPU tensors, float64 verts, oversized
+meshes, an unknown Laplacian method, for which the original raises) goes to the originals.
 """
 import importlib
 import types
@@ -105,6 +115,8 @@ _CLIP_FUNCTIONS = ("clip_faces", "convert_clipped_rasterization_to_original_face
 _NORMALS_MODULE = "pytorch3d.ops.mesh_face_areas_normals"
 _NORMALS_OPS = ("face_areas_normals_forward", "face_areas_normals_backward")
 _MESHES_MODULE = "pytorch3d.structures.meshes"
+_LOSS_PACKAGE = "pytorch3d.loss"
+_LOSS_FUNCTIONS = ("mesh_edge_loss", "mesh_laplacian_smoothing", "mesh_normal_consistency")
 _saved = {}
 # (module name, attribute) -> original (install_blending, install_splatter, install_shading, install_gouraud,
 # install_clipping and install_normals)
@@ -550,9 +562,62 @@ def install_normals():
     return [_NORMALS_MODULE, _MESHES_MODULE]
 
 
+def _regularizer_fused(meshes):
+    """Whether the fused regularisers take this batch: at least one mesh, float32 CUDA verts and int64 CUDA faces on
+    one device, V < 2^31 - 1 and 6F < 2^31."""
+    if len(meshes) == 0:
+        return False
+    verts, faces = meshes.verts_packed(), meshes.faces_packed()
+    return _mesh_fused(verts, faces) and 6 * faces.shape[0] < (1 << 31)
+
+
+def _regularizer_dispatch(name, original):
+    from . import regularizers as ours
+
+    if name == "mesh_edge_loss":
+        def mesh_edge_loss(meshes, target_length: float = 0.0):
+            if _regularizer_fused(meshes):
+                return ours.mesh_edge_loss(meshes, target_length)
+            return original(meshes, target_length)
+        fn = mesh_edge_loss
+    elif name == "mesh_laplacian_smoothing":
+        def mesh_laplacian_smoothing(meshes, method: str = "uniform"):
+            if method in _b200_C.LAPLACIAN_METHODS and _regularizer_fused(meshes):
+                return ours.mesh_laplacian_smoothing(meshes, method)
+            return original(meshes, method)
+        fn = mesh_laplacian_smoothing
+    else:
+        def mesh_normal_consistency(meshes):
+            if _regularizer_fused(meshes):
+                return ours.mesh_normal_consistency(meshes)
+            return original(meshes)
+        fn = mesh_normal_consistency
+    fn.__doc__ = original.__doc__
+    return fn
+
+
+def install_regularizers():
+    """Patch PyTorch3D's mesh regularisers (must be importable): `mesh_edge_loss`, `mesh_laplacian_smoothing` and
+    `mesh_normal_consistency` in pytorch3d.loss and in their defining modules pytorch3d.loss.<name>.  Returns the list
+    of patched module names."""
+    patched = [_LOSS_PACKAGE]
+    package = importlib.import_module(_LOSS_PACKAGE)
+    for name in _LOSS_FUNCTIONS:
+        modname = _LOSS_PACKAGE + "." + name
+        module = importlib.import_module(modname)
+        original = module.__dict__[name]
+        for owner, key in ((module, modname), (package, _LOSS_PACKAGE)):
+            if (key, name) not in _saved_blend:
+                _saved_blend[(key, name)] = owner.__dict__[name]
+                setattr(owner, name, _regularizer_dispatch(name, original))
+        patched.append(modname)
+    return patched
+
+
 def uninstall():
     """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_gouraud()`,
-    `install_textures()`, `install_texture_atlas()`, `install_clipping()` and `install_normals()`."""
+    `install_textures()`, `install_texture_atlas()`, `install_clipping()`, `install_normals()` and
+    `install_regularizers()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
