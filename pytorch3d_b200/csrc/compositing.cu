@@ -25,6 +25,30 @@ struct Strides4 {
 
 constexpr float kCompEps = 1e-9f;  // alpha_composite.cu:20
 
+// The backward kernels carry the transmittance as m * 2^e (e <= 0, a multiple of 64): the product of K factors
+// (1 - alpha) underflows float32 for long or opaque chains (150 uniform alphas, or ten at 1 - 6e-6), and the exclusive
+// prefixes recovered from it by division would then be 0 or wrong.  Rescaling by 2^64 is exact, so a pixel whose
+// product stays above 2^-64 computes exactly what it would with a plain float (e == 0 throughout).  For alphas in
+// [0, 1], |1 - alpha| >= 2^-24 unless it is 0, so m stays a normal float in [2^-88, 1) whenever e < 0.
+__device__ __forceinline__ void trans_mul(float& m, int& e, float f) {
+  m *= f;
+  if (fabsf(m) < 0x1p-64f && m != 0.0f) {
+    m *= 0x1p64f;
+    e -= 64;
+  }
+}
+__device__ __forceinline__ void trans_div(float& m, int& e, float f) {
+  m /= f;
+  if (e < 0 && fabsf(m) >= 1.0f) {
+    m *= 0x1p-64f;
+    e += 64;
+  }
+}
+// m * 2^e rounded to a float: subnormal below 2^-126, 0 below 2^-150
+__device__ __forceinline__ float trans_value(float m, int e) {
+  return e == 0 ? m : e == -64 ? m * 0x1p-64f : e == -128 ? m * 0x1p-128f : 0.0f;
+}
+
 // One 16-byte reduction for the four channels of a point (point-major features, C = 4): sm_90+ vector atomics.
 __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
@@ -101,9 +125,10 @@ __global__ void __launch_bounds__(256)
     // transmittance before the last valid slot, then walk the slots backwards keeping the suffix sum
     //   S_k = sum_{t>k} cum_t * alpha_t * A_t,   A_t = sum_c grad_out_c * feat[c, idx_t]
     // grad_alpha_k = cum_k * A_k - S_k / (1 - alpha_k + eps)          (alpha_composite.cu:112-134, summed over c)
-    float cum = 1.0f;
+    float cum = 1.0f;  // transmittance cum * 2^e (trans_mul)
+    int e = 0;
     for (int k = 0; k < K; ++k) {
-      if (ip[k * si.k] >= 0) cum *= 1.0f - ap[k * sa.k];
+      if (ip[k * si.k] >= 0) trans_mul(cum, e, 1.0f - ap[k * sa.k]);
     }
     float suffix = 0.0f;
     for (int k = K - 1; k >= 0; --k) {
@@ -116,16 +141,19 @@ __global__ void __launch_bounds__(256)
       const float one_minus = 1.0f - a;
       // cum currently includes slot k: undo it (exactly what the forward chain had before slot k, up to rounding;
       // recomputed from scratch when the factor is ~0 to avoid dividing by it)
-      float cum_k;
+      float cum_k = cum;
+      int e_k = e;
       if (fabsf(one_minus) > 1e-6f) {
-        cum_k = cum / one_minus;
+        trans_div(cum_k, e_k, one_minus);
       } else {
         cum_k = 1.0f;
+        e_k = 0;
         for (int l = 0; l < k; ++l)
-          if (ip[l * si.k] >= 0) cum_k *= 1.0f - ap[l * sa.k];
+          if (ip[l * si.k] >= 0) trans_mul(cum_k, e_k, 1.0f - ap[l * sa.k]);
       }
+      const float t_k = trans_value(cum_k, e_k);
       float A = 0.0f;
-      const float w = cum_k * a;
+      const float w = t_k * a;
       if (pm4) {  // point-major features, four channels: one 16-byte load and one 16-byte reduction per hit
         const float4 f = __ldg(reinterpret_cast<const float4*>(features) + id);
         const float g0 = go[0], g1 = go[plane], g2 = go[2 * plane], g3 = go[3 * plane];
@@ -138,9 +166,10 @@ __global__ void __launch_bounds__(256)
           atomicAdd(grad_features + c * fs_c + id * fs_p, g * w);  // (:115-117)
         }
       }
-      ga[k * plane] = cum_k * A - suffix / (one_minus + kCompEps);
+      ga[k * plane] = t_k * A - suffix / (one_minus + kCompEps);
       suffix += w * A;
       cum = cum_k;
+      e = e_k;
     }
   }
 }
@@ -337,8 +366,9 @@ __global__ void __launch_bounds__(256)
     }
     // (the arithmetic of alpha_composite_backward_kernel above, with alpha_k = 1 - d_k * inv)
     float cum = 1.0f;
+    int e = 0;
     for (int k = 0; k < K; ++k)
-      if (ip[k] >= 0) cum *= 1.0f - fsub(1.0f, fmul(dp[k], inv));
+      if (ip[k] >= 0) trans_mul(cum, e, 1.0f - fsub(1.0f, fmul(dp[k], inv)));
     float suffix = 0.0f;
     for (int k = K - 1; k >= 0; --k) {
       const int id = ip[k];
@@ -348,16 +378,19 @@ __global__ void __launch_bounds__(256)
       }
       const float a = fsub(1.0f, fmul(dp[k], inv));
       const float one_minus = 1.0f - a;
-      float cum_k;
+      float cum_k = cum;
+      int e_k = e;
       if (fabsf(one_minus) > 1e-6f) {
-        cum_k = cum / one_minus;
+        trans_div(cum_k, e_k, one_minus);
       } else {
         cum_k = 1.0f;
+        e_k = 0;
         for (int l = 0; l < k; ++l)
-          if (ip[l] >= 0) cum_k *= 1.0f - fsub(1.0f, fmul(dp[l], inv));
+          if (ip[l] >= 0) trans_mul(cum_k, e_k, 1.0f - fsub(1.0f, fmul(dp[l], inv)));
       }
+      const float t_k = trans_value(cum_k, e_k);
       float A = 0.0f;
-      const float w = cum_k * a;
+      const float w = t_k * a;
       if (CMAX > 0) {
         float f[CMAX > 0 ? CMAX : 1];
         if (vec4) {
@@ -383,10 +416,11 @@ __global__ void __launch_bounds__(256)
           atomicAdd(grad_features + c * fs_c + id * fs_p, gc * w);
         }
       }
-      const float ga = cum_k * A - suffix / (one_minus + kCompEps);
+      const float ga = t_k * A - suffix / (one_minus + kCompEps);
       gd[k] = fmul(-ga, inv);  // d(1 - d * inv) / dd = -inv
       suffix += w * A;
       cum = cum_k;
+      e = e_k;
     }
   }
 }
