@@ -281,6 +281,30 @@ int b200r_softmax_rgb_blend_backward(const float* grad_out, const float* colors,
                                      float* grad_colors, float* grad_dists, float* grad_zbuf, void* stream);
 
 /*
+ * Fused depth shading (additional entry points, no counterpart in pytorch3d._C): the torch chains of
+ * pytorch3d/renderer/mesh/shader.py SoftDepthShader.forward and HardDepthShader.forward, one kernel per direction, on
+ * the rasterizer's layout (DESIGN.md section 19).
+ *  pix_to_face int64 (N,H,W,K) (valid where >= 0); zbuf, dists float32 (N,H,W,K); 1 <= K <= 150.
+ *  zfar: device float32, one value, or NULL and then the number zfar_value.
+ *  Soft: out float32 (N,H,W,1), fully written: sum_k w_k depth_k over the K slots and a last one of probability 1 at
+ *  depth zfar, w_k the differences of the prefix sums of sigmoid(-dists / sigma) * [valid] clamped to 1.
+ *  Backward: grad_out float32 (N,H,W,1); grad_zbuf and grad_dists float32 (N,H,W,K), fully written, no atomics.
+ *  Hard: out float32 (N,H,W,1), fully written: zbuf of slot 0 where pix_to_face of slot 0 is valid, zfar elsewhere.
+ *  Backward: grad_out float32 (N,H,W,1); grad_zbuf float32 (N,H,W,K), fully written (0 outside valid slots 0).
+ */
+int b200r_soft_depth_blend_forward(const int64_t* pix_to_face, const float* zbuf, const float* dists, int32_t N,
+                                   int32_t H, int32_t W, int32_t K, float sigma, const float* zfar, float zfar_value,
+                                   float* out, void* stream);
+int b200r_soft_depth_blend_backward(const float* grad_out, const int64_t* pix_to_face, const float* zbuf,
+                                    const float* dists, int32_t N, int32_t H, int32_t W, int32_t K, float sigma,
+                                    const float* zfar, float zfar_value, float* grad_zbuf, float* grad_dists,
+                                    void* stream);
+int b200r_hard_depth_forward(const int64_t* pix_to_face, const float* zbuf, int32_t N, int32_t H, int32_t W, int32_t K,
+                             const float* zfar, float zfar_value, float* out, void* stream);
+int b200r_hard_depth_backward(const float* grad_out, const int64_t* pix_to_face, int32_t N, int32_t H, int32_t W,
+                              int32_t K, float* grad_zbuf, void* stream);
+
+/*
  * Fused splatter blending (additional entry points, no counterpart in pytorch3d._C): what
  * pytorch3d/renderer/splatter_blend.py SplatterBlender.forward computes after its projection step, in one kernel for
  * the forward and two for the backward (DESIGN.md section 11).

@@ -541,6 +541,107 @@ def softmax_rgb_blend_backward(grad_out: torch.Tensor, colors: torch.Tensor, pix
     return grad_colors, grad_dists, grad_zbuf
 
 
+def _depth_zfar_arg(dev, zfar):
+    """(zfar ptr, zfar value, tensor to keep alive).  A 1-element float32 tensor on `dev` is read on the device; a
+    Python number goes to the kernel as a number."""
+    if torch.is_tensor(zfar):
+        if zfar.device != dev or zfar.dtype != torch.float32 or zfar.numel() != 1:
+            raise RuntimeError("zfar must be a number or a 1-element float32 tensor on %s" % dev)
+        z = zfar.reshape(1).contiguous()
+        return z.data_ptr(), 0.0, z
+    return None, float(zfar), None
+
+
+def _check_depth_inputs(pix_to_face, named_floats):
+    dev = _check_blend_inputs(named_floats, pix_to_face)
+    for name, t in named_floats:
+        if t.shape != pix_to_face.shape:
+            raise RuntimeError("pix_to_face and %s must both be (N, H, W, K)" % name)
+    if not 1 <= pix_to_face.shape[3] <= kMaxPointsPerPixel:
+        raise RuntimeError("Must have 1 <= faces_per_pixel <= %d" % kMaxPointsPerPixel)
+    return dev
+
+
+def _check_depth_grad(grad_out, pix_to_face):
+    _require_cuda(("grad_out", grad_out), ("pix_to_face", pix_to_face))
+    if grad_out.dtype != torch.float32 or tuple(grad_out.shape) != tuple(pix_to_face.shape[:3]) + (1,):
+        raise RuntimeError("grad_out must be a float32 tensor of shape (N, H, W, 1)")
+
+
+def soft_depth_blend(pix_to_face: torch.Tensor, zbuf: torch.Tensor, dists: torch.Tensor, sigma: float, zfar):
+    """Fused SoftDepthShader of pytorch3d/renderer/mesh/shader.py on the rasterizer's layout (no counterpart in
+    pytorch3d._C): pix_to_face (N,H,W,K) i64, zbuf / dists (N,H,W,K) f32, 1 <= K <= 150; zfar a number or a 1-element
+    float32 tensor on the same device -> (N,H,W,1) f32."""
+    dev = _check_depth_inputs(pix_to_face, [("zbuf", zbuf), ("dists", dists)])
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    zf_ptr, zf, keep = _depth_zfar_arg(dev, zfar)
+    p2f, zb, dd = pix_to_face.contiguous(), zbuf.contiguous(), dists.contiguous()
+    with torch.cuda.device(dev):
+        out = torch.empty((N, H, W, 1), dtype=torch.float32, device=dev)
+        if out.numel() == 0:
+            return out
+        _lib.check(lib.b200r_soft_depth_blend_forward(_ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K, float(sigma), zf_ptr,
+                                                      zf, _ptr(out), _stream_ptr(dev)))
+    del keep
+    return out
+
+
+def soft_depth_blend_backward(grad_out: torch.Tensor, pix_to_face: torch.Tensor, zbuf: torch.Tensor,
+                              dists: torch.Tensor, sigma: float, zfar):
+    """Backward of `soft_depth_blend` -> (grad_zbuf (N,H,W,K), grad_dists (N,H,W,K))."""
+    dev = _check_depth_inputs(pix_to_face, [("zbuf", zbuf), ("dists", dists)])
+    _check_depth_grad(grad_out, pix_to_face)
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    zf_ptr, zf, keep = _depth_zfar_arg(dev, zfar)
+    go, p2f, zb, dd = grad_out.contiguous(), pix_to_face.contiguous(), zbuf.contiguous(), dists.contiguous()
+    with torch.cuda.device(dev):
+        grad_zbuf = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
+        grad_dists = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
+        if grad_zbuf.numel() == 0:
+            return grad_zbuf, grad_dists
+        _lib.check(lib.b200r_soft_depth_blend_backward(_ptr(go), _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K,
+                                                       float(sigma), zf_ptr, zf, _ptr(grad_zbuf), _ptr(grad_dists),
+                                                       _stream_ptr(dev)))
+    del keep
+    return grad_zbuf, grad_dists
+
+
+def hard_depth(pix_to_face: torch.Tensor, zbuf: torch.Tensor, zfar):
+    """Fused HardDepthShader of pytorch3d/renderer/mesh/shader.py: zbuf of slot 0 where pix_to_face of slot 0 is valid,
+    zfar elsewhere.  pix_to_face (N,H,W,K) i64, zbuf (N,H,W,K) f32; zfar as for `soft_depth_blend` -> (N,H,W,1) f32."""
+    dev = _check_depth_inputs(pix_to_face, [("zbuf", zbuf)])
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    zf_ptr, zf, keep = _depth_zfar_arg(dev, zfar)
+    p2f, zb = pix_to_face.contiguous(), zbuf.contiguous()
+    with torch.cuda.device(dev):
+        out = torch.empty((N, H, W, 1), dtype=torch.float32, device=dev)
+        if out.numel() == 0:
+            return out
+        _lib.check(lib.b200r_hard_depth_forward(_ptr(p2f), _ptr(zb), N, H, W, K, zf_ptr, zf, _ptr(out),
+                                                _stream_ptr(dev)))
+    del keep
+    return out
+
+
+def hard_depth_backward(grad_out: torch.Tensor, pix_to_face: torch.Tensor):
+    """Backward of `hard_depth` -> grad_zbuf (N,H,W,K): grad_out on slot 0 of valid pixels, 0 everywhere else."""
+    _check_depth_inputs(pix_to_face, [])
+    _check_depth_grad(grad_out, pix_to_face)
+    lib = _lib.load()
+    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    go, p2f = grad_out.contiguous(), pix_to_face.contiguous()
+    dev = pix_to_face.device
+    with torch.cuda.device(dev):
+        grad_zbuf = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
+        if grad_zbuf.numel() == 0:
+            return grad_zbuf
+        _lib.check(lib.b200r_hard_depth_backward(_ptr(go), _ptr(p2f), N, H, W, K, _ptr(grad_zbuf), _stream_ptr(dev)))
+    return grad_zbuf
+
+
 def _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma):
     dev = _check_blend_inputs([("colors", colors), ("pixel_coords_screen", pixel_coords_screen)], background_mask,
                               "background_mask", torch.bool)

@@ -68,6 +68,12 @@ SIGNATURES = {
     "b200r_softmax_rgb_blend_backward": (
         ctypes.c_int,
         [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _vp, _vp, _vp, _vp, _f64, _f64, _vp, _vp, _vp, _vp]),
+    "b200r_soft_depth_blend_forward": (
+        ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _f32, _vp, _vp]),
+    "b200r_soft_depth_blend_backward": (
+        ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _f32, _vp, _vp, _vp]),
+    "b200r_hard_depth_forward": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _f32, _vp, _vp]),
+    "b200r_hard_depth_backward": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
     "b200r_splatter_blend_forward": (
         ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _f64, _vp, _vp, _vp, _vp]),
     "b200r_splatter_blend_workspace_bytes": (_sz, [_i32, _i32, _i32]),

@@ -1,9 +1,11 @@
 """Mesh blending (SURVEY.md 8f-5), same API as the reference's pytorch3d/renderer/blending.py: `BlendParams`,
-`hard_rgb_blend`, `sigmoid_alpha_blend` and `softmax_rgb_blend`.
+`hard_rgb_blend`, `sigmoid_alpha_blend` and `softmax_rgb_blend`; and the depth blends of the reference's
+SoftDepthShader and HardDepthShader (pytorch3d/renderer/mesh/shader.py): `soft_depth` and `hard_depth`.
 
 `sigmoid_alpha_blend` runs the drop-in `_C.sigmoid_alpha_blend[_backward]` kernels (bit-identical to the reference's);
 `softmax_rgb_blend` runs one fused kernel per direction instead of the reference's chain of some twenty torch kernels;
-`hard_rgb_blend` needs no kernel of its own.  None of them synchronises the host.
+`hard_rgb_blend` needs no kernel of its own; `soft_depth` and `hard_depth` run one fused kernel per direction (DESIGN.md
+section 19).  None of them synchronises the host.
 """
 from typing import NamedTuple, Sequence, Union
 
@@ -110,3 +112,57 @@ def softmax_rgb_blend(colors: torch.Tensor, fragments, blend_params: BlendParams
     return _SoftmaxRGBBlend.apply(colors, fragments.zbuf, fragments.dists, fragments.pix_to_face,
                                   float(blend_params.sigma), float(blend_params.gamma), background,
                                   _as_device_float(znear, device), _as_device_float(zfar, device))
+
+
+def _check_zfar(zfar, fn):
+    if torch.is_tensor(zfar) and zfar.requires_grad:
+        raise ValueError("%s: zfar must not require grad (gradients flow to zbuf and dists only)" % fn)
+
+
+class _SoftDepth(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, zbuf, dists, pix_to_face, sigma, zfar):
+        out = _C.soft_depth_blend(pix_to_face, zbuf, dists, sigma, zfar)
+        ctx.save_for_backward(zbuf, dists, pix_to_face)
+        ctx.args = (sigma, zfar)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        zbuf, dists, pix_to_face = ctx.saved_tensors
+        grad_zbuf, grad_dists = _C.soft_depth_blend_backward(grad_out, pix_to_face, zbuf, dists, *ctx.args)
+        return grad_zbuf, grad_dists, None, None, None
+
+
+def soft_depth(fragments, sigma: float, zfar: Union[float, torch.Tensor]) -> torch.Tensor:
+    """Depth blended over the K faces of each pixel and a background at `zfar` -- the reference's SoftDepthShader.
+    Each face's coverage is sigmoid(-dists / sigma) (0 for empty slots); the faces are taken nearest first until their
+    cumulative coverage reaches 1, and the background gets what is left.
+
+    `fragments` with pix_to_face, zbuf and dists (N,H,W,K), 1 <= K <= 150; zfar a number or a 1-element float32 tensor
+    on the same device (read on the device).  Returns (N,H,W,1).  Gradients flow to `fragments.zbuf` and
+    `fragments.dists`; a zfar that requires grad raises ValueError.
+    """
+    _check_zfar(zfar, "soft_depth")
+    return _SoftDepth.apply(fragments.zbuf, fragments.dists, fragments.pix_to_face, float(sigma), zfar)
+
+
+class _HardDepth(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, zbuf, pix_to_face, zfar):
+        out = _C.hard_depth(pix_to_face, zbuf, zfar)
+        ctx.save_for_backward(pix_to_face)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        pix_to_face, = ctx.saved_tensors
+        return _C.hard_depth_backward(grad_out, pix_to_face), None, None
+
+
+def hard_depth(fragments, zfar: Union[float, torch.Tensor]) -> torch.Tensor:
+    """Depth of the closest face, `zfar` where no face covers the pixel -- the reference's HardDepthShader.
+    `fragments` with pix_to_face and zbuf (N,H,W,K), 1 <= K <= 150; zfar as for `soft_depth`.  Returns (N,H,W,1);
+    the gradient flows to slot 0 of `fragments.zbuf` on covered pixels."""
+    _check_zfar(zfar, "hard_depth")
+    return _HardDepth.apply(fragments.zbuf, fragments.pix_to_face, zfar)

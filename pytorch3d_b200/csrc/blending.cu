@@ -32,6 +32,12 @@
 //    atomics.
 //    K buckets: K <= 8 runs one thread per pixel with the slots in registers (16-byte loads and stores when K = 8);
 //    8 < K <= 150 runs one warp per pixel, lane k % 32 holding slot k in registers, all accesses coalesced.
+//
+// 3. SoftDepthShader / HardDepthShader forward / backward (no counterpart in pytorch3d._C; DESIGN.md section 19): the
+//    torch chains of pytorch3d/renderer/mesh/shader.py, one kernel per direction, in the same K buckets as 2.
+//      p_k = softmax_prob(d_k) * v_k (k < K), p_K = 1;  c_k = sum_{j <= k} p_j;  w_k = min(c_k, 1) - min(c_{k-1}, 1)
+//      out = sum_{k <= K} w_k depth_k  (depth_K = zfar)
+//    Only the order of the prefix sum and of the sum over k differs from torch's cumsum and sum.
 #include "common.cuh"
 #include "raster_math.cuh"
 
@@ -142,8 +148,8 @@ __device__ __forceinline__ void store4(float* p, float4 v, bool vec) {
 }
 
 // Loads of one pixel's K slots.  Register bucket (KMAX > 0): all K <= KMAX slots at once, 16-byte loads when
-// K == KMAX == 8 and the rows are 16-byte aligned.
-template <int KMAX>
+// K == KMAX == 8 and the rows are 16-byte aligned.  COLORS = false leaves out the colours (depth blending).
+template <int KMAX, bool COLORS = true>
 struct SlotCache {
   float c[KMAX][3], d[KMAX], z[KMAX], v[KMAX];
 
@@ -158,7 +164,9 @@ struct SlotCache {
 #pragma unroll
     for (int k = 0; k < KMAX; ++k) {
       if (k < K) {
-        c[k][0] = __ldg(cp + 3 * k); c[k][1] = __ldg(cp + 3 * k + 1); c[k][2] = __ldg(cp + 3 * k + 2);
+        if constexpr (COLORS) {
+          c[k][0] = __ldg(cp + 3 * k); c[k][1] = __ldg(cp + 3 * k + 1); c[k][2] = __ldg(cp + 3 * k + 2);
+        }
         d[k] = __ldg(dp + k);
         z[k] = __ldg(zp + k);
         v[k] = __ldg(fp + k) >= 0 ? 1.0f : 0.0f;
@@ -170,11 +178,13 @@ struct SlotCache {
   __device__ __forceinline__ void store(float* cp, float* dp, float* zp, int K, bool vec) {
     if constexpr (KMAX == 8) {
       if (vec) {
-        float4* c4 = reinterpret_cast<float4*>(cp);
+        if constexpr (COLORS) {
+          float4* c4 = reinterpret_cast<float4*>(cp);
 #pragma unroll
-        for (int i = 0; i < 6; ++i)
-          c4[i] = make_float4(c[(4 * i) / 3][(4 * i) % 3], c[(4 * i + 1) / 3][(4 * i + 1) % 3],
-                              c[(4 * i + 2) / 3][(4 * i + 2) % 3], c[(4 * i + 3) / 3][(4 * i + 3) % 3]);
+          for (int i = 0; i < 6; ++i)
+            c4[i] = make_float4(c[(4 * i) / 3][(4 * i) % 3], c[(4 * i + 1) / 3][(4 * i + 1) % 3],
+                                c[(4 * i + 2) / 3][(4 * i + 2) % 3], c[(4 * i + 3) / 3][(4 * i + 3) % 3]);
+        }
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           reinterpret_cast<float4*>(dp)[i] = make_float4(d[4 * i], d[4 * i + 1], d[4 * i + 2], d[4 * i + 3]);
@@ -186,7 +196,9 @@ struct SlotCache {
 #pragma unroll
     for (int k = 0; k < KMAX; ++k) {
       if (k < K) {
-        cp[3 * k] = c[k][0]; cp[3 * k + 1] = c[k][1]; cp[3 * k + 2] = c[k][2];
+        if constexpr (COLORS) {
+          cp[3 * k] = c[k][0]; cp[3 * k + 1] = c[k][1]; cp[3 * k + 2] = c[k][2];
+        }
         dp[k] = d[k];
         zp[k] = z[k];
       }
@@ -197,13 +209,15 @@ struct SlotCache {
   // two 16-byte loads.
   __device__ __forceinline__ void load_vec8(const float* cp, const int64_t* fp, const float* zp, const float* dp) {
     {
-      const float4* c4 = reinterpret_cast<const float4*>(cp);
+      if constexpr (COLORS) {
+        const float4* c4 = reinterpret_cast<const float4*>(cp);
 #pragma unroll
-      for (int i = 0; i < 6; ++i) {
-        const float4 t = __ldg(c4 + i);
-        const float tt[4] = {t.x, t.y, t.z, t.w};
+        for (int i = 0; i < 6; ++i) {
+          const float4 t = __ldg(c4 + i);
+          const float tt[4] = {t.x, t.y, t.z, t.w};
 #pragma unroll
-        for (int j = 0; j < 4; ++j) c[(4 * i + j) / 3][(4 * i + j) % 3] = tt[j];
+          for (int j = 0; j < 4; ++j) c[(4 * i + j) / 3][(4 * i + j) % 3] = tt[j];
+        }
       }
       const float4* d4 = reinterpret_cast<const float4*>(dp);
       const float4* z4 = reinterpret_cast<const float4*>(zp);
@@ -394,6 +408,56 @@ __device__ __forceinline__ float warp_prod(float v) {
   return v;
 }
 
+// Scans of x under `op` (associative and commutative, identity `id`) over a pixel's slots, x_of(j) the value of slot
+// 32 j + lane:
+// Hillis-Steele scans inside each row of 32 slots, the row totals carried across the rows.
+//   UP:   up[j] = op over the slots <= k,  pre[j] = op over the slots < k  (id at slot 0)
+//   DOWN: down[j] = op over the slots >= k, suf[j] = op over the slots > k  (id at the last slot of the last row)
+// pre at slot k holds the bits of up at slot k - 1, suf at slot k those of down at slot k + 1.
+template <int NS, bool UP, bool DOWN, typename X, typename Op>
+__device__ __forceinline__ void warp_scans(X&& x_of, int lane, float id, Op op, float (&up)[NS],
+                                           float (&pre)[NS], float (&down)[NS], float (&suf)[NS]) {
+  float total[NS];
+#pragma unroll
+  for (int j = 0; j < NS; ++j) {
+    const float x = x_of(j);
+    float u = x, d = x;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      float a = id, b = id;
+      if constexpr (UP) a = __shfl_up_sync(kFullMask, u, o);
+      if constexpr (DOWN) b = __shfl_down_sync(kFullMask, d, o);
+      if (UP && lane >= o) u = op(u, a);
+      if (DOWN && lane + o < 32) d = op(d, b);
+    }
+    total[j] = UP ? __shfl_sync(kFullMask, u, 31) : __shfl_sync(kFullMask, d, 0);
+    if constexpr (UP) pre[j] = __shfl_up_sync(kFullMask, u, 1);
+    if constexpr (DOWN) suf[j] = __shfl_down_sync(kFullMask, d, 1);
+    if (UP && lane == 0) pre[j] = id;
+    if (DOWN && lane == 31) suf[j] = id;
+    up[j] = u;
+    down[j] = d;
+  }
+  if constexpr (UP) {
+    float before = id;
+#pragma unroll
+    for (int j = 0; j < NS; ++j) {
+      pre[j] = op(pre[j], before);
+      up[j] = op(up[j], before);
+      before = op(before, total[j]);
+    }
+  }
+  if constexpr (DOWN) {
+    float after = id;
+#pragma unroll
+    for (int j = NS - 1; j >= 0; --j) {
+      suf[j] = op(suf[j], after);
+      down[j] = op(down[j], after);
+      after = op(after, total[j]);
+    }
+  }
+}
+
 template <int NS, bool BACKWARD>
 __global__ void __launch_bounds__(256)
     softmax_rgb_blend_warp_kernel(const float* __restrict__ grad_out, const float* __restrict__ colors,
@@ -471,36 +535,10 @@ __global__ void __launch_bounds__(256)
       const float4 g = load4(grad_out + 4 * pix, io4);
       const float inv_D = 1.0f / D;
       const float dzdz = dzinv_dz(zm);
-      // exclusive prefix / suffix products of (1 - p): scans inside each row of 32 slots, row totals across rows
-      float pre[NS], suf[NS], total[NS];
-#pragma unroll
-      for (int j = 0; j < NS; ++j) {
-        const float x = 32 * j + lane < K ? 1.0f - pt[j] * v[j] : 1.0f;
-        float up = x, down = x;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const float a = __shfl_up_sync(kFullMask, up, o), b = __shfl_down_sync(kFullMask, down, o);
-          if (lane >= o) up *= a;
-          if (lane + o < 32) down *= b;
-        }
-        total[j] = __shfl_sync(kFullMask, up, 31);
-        pre[j] = __shfl_up_sync(kFullMask, up, 1);
-        suf[j] = __shfl_down_sync(kFullMask, down, 1);
-        if (lane == 0) pre[j] = 1.0f;
-        if (lane == 31) suf[j] = 1.0f;
-      }
-      float before = 1.0f;
-#pragma unroll
-      for (int j = 0; j < NS; ++j) {
-        pre[j] *= before;
-        before *= total[j];
-      }
-      float after = 1.0f;
-#pragma unroll
-      for (int j = NS - 1; j >= 0; --j) {
-        suf[j] *= after;
-        after *= total[j];
-      }
+      // exclusive prefix / suffix products of (1 - p)
+      float up[NS], pre[NS], down[NS], suf[NS];
+      warp_scans<NS, true, true>([&](int j) { return 32 * j + lane < K ? 1.0f - pt[j] * v[j] : 1.0f; }, lane, 1.0f,
+                                 [](float a, float b) { return a * b; }, up, pre, down, suf);
       float sum_qw = 0.0f, dz_arg = 0.0f;
       float gz[NS];
 #pragma unroll
@@ -539,6 +577,165 @@ __global__ void __launch_bounds__(256)
         if (k < K) grad_zbuf[pix * K + k] = gz[j];
       }
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ depth
+// zfar of the depth shaders: a device float (a 1-element tensor, read in the kernel) or, when null, a number.
+struct DepthFar {
+  const float* ptr;
+  float value;
+};
+
+__device__ __forceinline__ float zfar_of(const DepthFar& f) { return f.ptr ? __ldg(f.ptr) : f.value; }
+
+// clamp(max=1), which lets a NaN through
+__device__ __forceinline__ float clamp1(float c) { return c > 1.0f ? 1.0f : c; }
+
+// ---- K <= 8: one thread per pixel, the slots in registers, the prefix sums in ascending k.  Slot K (p = 1, depth
+// zfar) follows the loop.
+template <int KMAX>
+__global__ void __launch_bounds__(256)
+    soft_depth_forward_kernel(const int64_t* __restrict__ pix_to_face, const float* __restrict__ zbuf,
+                              const float* __restrict__ dists, int64_t P, int K, float inv_sigma, DepthFar far,
+                              float* __restrict__ out) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const bool vec = K == 8 && aligned16(pix_to_face) && aligned16(zbuf) && aligned16(dists);
+  const float zf = zfar_of(far);
+  for (int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pix < P; pix += stride) {
+    SlotCache<KMAX, false> sc;
+    sc.load(nullptr, pix_to_face + pix * K, zbuf + pix * K, dists + pix * K, K, vec);
+    float c = 0.0f, prev = 0.0f, acc = 0.0f;
+    for_slots<KMAX>(K, [&](int k) {
+      c = fadd(c, fmul(softmax_prob(sc.d[k], inv_sigma), sc.v[k]));
+      const float ct = clamp1(c);
+      acc = fadd(acc, fmul(fsub(ct, prev), sc.z[k]));
+      prev = ct;
+    });
+    out[pix] = fadd(acc, fmul(fsub(clamp1(fadd(c, 1.0f)), prev), zf));
+  }
+}
+
+template <int KMAX>
+__global__ void __launch_bounds__(256)
+    soft_depth_backward_kernel(const float* __restrict__ grad_out, const int64_t* __restrict__ pix_to_face,
+                               const float* __restrict__ zbuf, const float* __restrict__ dists, int64_t P, int K,
+                               float inv_sigma, DepthFar far, float* __restrict__ grad_zbuf,
+                               float* __restrict__ grad_dists) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const bool vec = K == 8 && aligned16(pix_to_face) && aligned16(zbuf) && aligned16(dists) &&
+                   aligned16(grad_zbuf) && aligned16(grad_dists);
+  const float zf = zfar_of(far);
+  for (int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pix < P; pix += stride) {
+    SlotCache<KMAX, false> sc;
+    sc.load(nullptr, pix_to_face + pix * K, zbuf + pix * K, dists + pix * K, K, vec);
+    const float g = __ldg(grad_out + pix);
+    float s[KMAX], cs[KMAX];  // sigmoids and prefix sums c_k
+    float c = 0.0f;
+    for_slots<KMAX>(K, [&](int k) {
+      s[k] = softmax_prob(sc.d[k], inv_sigma);
+      c = fadd(c, fmul(s[k], sc.v[k]));
+      cs[k] = c;
+    });
+    // slot K: gw_K = g zfar, gc~_K = gw_K - 0; gp runs the suffix sums of gc from slot K down
+    float gw_next = fmul(g, zf);
+    float gp = fadd(c, 1.0f) <= 1.0f ? gw_next : 0.0f;
+    for_slots_reverse<KMAX>(K, [&](int k) {
+      const float gw = fmul(g, sc.z[k]);
+      gp = fadd(gp, cs[k] <= 1.0f ? fsub(gw, gw_next) : 0.0f);
+      gw_next = gw;
+      sc.z[k] = fmul(g, fsub(clamp1(cs[k]), k > 0 ? clamp1(cs[k > 0 ? k - 1 : 0]) : 0.0f));
+      sc.d[k] = -fmul(fmul(fmul(fmul(gp, sc.v[k]), fsub(1.0f, s[k])), s[k]), inv_sigma);
+    });
+    sc.store(nullptr, grad_dists + pix * K, grad_zbuf + pix * K, K, vec);
+  }
+}
+
+// ---- 8 < K <= 150: one warp per pixel, slot k on lane k % 32 of row k / 32, slot K (p = 1, depth zfar) included:
+// NS = ceil((K + 1) / 32) rows.  The prefix sums c_k and the suffix sums of the backward are warp_scans; c_{k-1}
+// is the exclusive prefix, which has the bits of c_{k-1} itself.
+// (4 blocks per SM: a 64-register budget, within which ptxas allocates the NS = 4 backward without the spill it
+// makes when left to its own target)
+template <int NS, bool BACKWARD>
+__global__ void __launch_bounds__(256, 4)
+    soft_depth_warp_kernel(const float* __restrict__ grad_out, const int64_t* __restrict__ pix_to_face,
+                           const float* __restrict__ zbuf, const float* __restrict__ dists, int64_t P, int K,
+                           float inv_sigma, DepthFar far, float* __restrict__ out, float* __restrict__ grad_zbuf,
+                           float* __restrict__ grad_dists) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * kWarpsPerBlock;
+  const float zf = zfar_of(far);
+  const auto add = [](float a, float b) { return fadd(a, b); };
+  for (int64_t pix = (int64_t)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5); pix < P; pix += warps) {
+    const int64_t base = pix * K;
+    float s[NS], v[NS], z[NS], p[NS];
+#pragma unroll
+    for (int j = 0; j < NS; ++j) {
+      const int k = 32 * j + lane;
+      const bool in = k < K;
+      v[j] = in && __ldg(pix_to_face + base + k) >= 0 ? 1.0f : 0.0f;
+      s[j] = softmax_prob(in ? __ldg(dists + base + k) : 0.0f, inv_sigma);
+      z[j] = in ? __ldg(zbuf + base + k) : (k == K ? zf : 0.0f);
+      p[j] = in ? fmul(s[j], v[j]) : (k == K ? 1.0f : 0.0f);
+    }
+    float c[NS], cprev[NS], down_unused[NS], suf_unused[NS];
+    warp_scans<NS, true, false>([&](int j) { return p[j]; }, lane, 0.0f, add, c, cprev, down_unused, suf_unused);
+    if constexpr (!BACKWARD) {
+      float acc = 0.0f;
+#pragma unroll
+      for (int j = 0; j < NS; ++j)
+        if (32 * j + lane <= K) acc = fadd(acc, fmul(fsub(clamp1(c[j]), clamp1(cprev[j])), z[j]));
+      acc = warp_sum(acc);
+      if (lane == 0) out[pix] = acc;
+    } else {
+      const float g = __ldg(grad_out + pix);
+      float gw[NS];
+#pragma unroll
+      for (int j = 0; j < NS; ++j) gw[j] = 32 * j + lane <= K ? fmul(g, z[j]) : 0.0f;
+      float gc[NS];
+#pragma unroll
+      for (int j = 0; j < NS; ++j) {  // gc_k = [c_k <= 1] (gw_k - gw_{k+1})
+        const float below = __shfl_down_sync(kFullMask, gw[j], 1);
+        const float next_row = __shfl_sync(kFullMask, gw[j + 1 < NS ? j + 1 : j], 0);
+        const float next = lane < 31 ? below : (j + 1 < NS ? next_row : 0.0f);
+        gc[j] = c[j] <= 1.0f ? fsub(gw[j], next) : 0.0f;
+      }
+      float up_unused[NS], pre_unused[NS], gp[NS];  // gp_k = sum of gc over the slots >= k
+      warp_scans<NS, false, true>([&](int j) { return gc[j]; }, lane, 0.0f, add, up_unused, pre_unused, gp,
+                                  suf_unused);
+#pragma unroll
+      for (int j = 0; j < NS; ++j) {
+        const int k = 32 * j + lane;
+        if (k < K) {
+          grad_zbuf[base + k] = fmul(g, fsub(clamp1(c[j]), clamp1(cprev[j])));
+          grad_dists[base + k] = -fmul(fmul(fmul(fmul(gp[j], v[j]), fsub(1.0f, s[j])), s[j]), inv_sigma);
+        }
+      }
+    }
+  }
+}
+
+// HardDepthShader: slot 0's depth on covered pixels, zfar elsewhere.  One thread per pixel.
+__global__ void __launch_bounds__(256)
+    hard_depth_forward_kernel(const int64_t* __restrict__ pix_to_face, const float* __restrict__ zbuf, int64_t P,
+                              int K, DepthFar far, float* __restrict__ out) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const float zf = zfar_of(far);
+  for (int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pix < P; pix += stride)
+    out[pix] = __ldg(pix_to_face + pix * K) >= 0 ? __ldg(zbuf + pix * K) : zf;
+}
+
+// The gradient of slot 0's depth on covered pixels; every other slot gets 0, written here (no zero-fill pass).  One
+// thread per slot, so that the stores of a warp are contiguous: a thread per pixel writing its K slots is several times
+// slower at large K (DESIGN.md section 19).
+__global__ void __launch_bounds__(256)
+    hard_depth_backward_kernel(const float* __restrict__ grad_out, const int64_t* __restrict__ pix_to_face, int64_t P,
+                               int K, float* __restrict__ grad_zbuf) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t total = P * K;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const int64_t pix = i / K;
+    grad_zbuf[i] = i == pix * K && __ldg(pix_to_face + i) >= 0 ? __ldg(grad_out + pix) : 0.0f;
   }
 }
 
@@ -665,4 +862,94 @@ extern "C" int b200r_softmax_rgb_blend_backward(const float* grad_out, const flo
   }
   return launch_warp_kernel<true>(grad_out, colors, pix_to_face, zbuf, dists, P, (int64_t)H * W, K, s, nullptr,
                                   grad_colors, grad_dists, grad_zbuf, stream);
+}
+
+static int depth_args(int32_t N, int32_t H, int32_t W, int32_t K) {
+  if (N < 0 || H < 0 || W < 0) return fail(B200R_ERR_INVALID_ARGUMENT, "negative size");
+  if (K < 1 || K > B200R_MAX_K) return fail(B200R_ERR_INVALID_ARGUMENT, "Must have 1 <= faces_per_pixel <= 150");
+  return B200R_OK;
+}
+
+// K > 8: one warp per pixel, NS = ceil((K + 1) / 32) rows of slots.
+template <bool BACKWARD>
+static int launch_depth_warp_kernel(const float* grad_out, const int64_t* pix_to_face, const float* zbuf,
+                                    const float* dists, int64_t P, int K, float inv_sigma, DepthFar far, float* out,
+                                    float* grad_zbuf, float* grad_dists, cudaStream_t stream) {
+  const unsigned blocks = (unsigned)cap_grid_stride_blocks((P + kWarpsPerBlock - 1) / kWarpsPerBlock);
+#define B200R_DEPTH_WARP(NS)                                                                                       \
+  soft_depth_warp_kernel<NS, BACKWARD><<<blocks, 32 * kWarpsPerBlock, 0, stream>>>(                               \
+      grad_out, pix_to_face, zbuf, dists, P, K, inv_sigma, far, out, grad_zbuf, grad_dists)
+  switch ((K + 32) / 32) {
+    case 1: B200R_DEPTH_WARP(1); break;
+    case 2: B200R_DEPTH_WARP(2); break;
+    case 3: B200R_DEPTH_WARP(3); break;
+    case 4: B200R_DEPTH_WARP(4); break;
+    default: B200R_DEPTH_WARP(5); break;  // K + 1 <= 151 (checked by the caller)
+  }
+#undef B200R_DEPTH_WARP
+  B200R_LAUNCHED(BACKWARD ? "soft_depth_warp_kernel<backward>" : "soft_depth_warp_kernel<forward>");
+  return B200R_OK;
+}
+
+extern "C" int b200r_soft_depth_blend_forward(const int64_t* pix_to_face, const float* zbuf, const float* dists,
+                                              int32_t N, int32_t H, int32_t W, int32_t K, float sigma,
+                                              const float* zfar, float zfar_value, float* out, void* stream_) {
+  const int rc = depth_args(N, H, W, K);
+  if (rc != B200R_OK) return rc;
+  const int64_t P = (int64_t)N * H * W;
+  if (P == 0) return B200R_OK;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const DepthFar far{zfar, zfar_value};
+  if (K <= 8) {
+    soft_depth_forward_kernel<8><<<(unsigned)blend_blocks(P, K, 0), 256, 0, stream>>>(pix_to_face, zbuf, dists, P,
+                                                                                      K, 1.0f / sigma, far, out);
+    B200R_LAUNCHED("soft_depth_forward_kernel");
+    return B200R_OK;
+  }
+  return launch_depth_warp_kernel<false>(nullptr, pix_to_face, zbuf, dists, P, K, 1.0f / sigma, far, out, nullptr,
+                                         nullptr, stream);
+}
+
+extern "C" int b200r_soft_depth_blend_backward(const float* grad_out, const int64_t* pix_to_face, const float* zbuf,
+                                               const float* dists, int32_t N, int32_t H, int32_t W, int32_t K,
+                                               float sigma, const float* zfar, float zfar_value, float* grad_zbuf,
+                                               float* grad_dists, void* stream_) {
+  const int rc = depth_args(N, H, W, K);
+  if (rc != B200R_OK) return rc;
+  const int64_t P = (int64_t)N * H * W;
+  if (P == 0) return B200R_OK;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const DepthFar far{zfar, zfar_value};
+  if (K <= 8) {
+    soft_depth_backward_kernel<8><<<(unsigned)blend_blocks(P, K, 0), 256, 0, stream>>>(
+        grad_out, pix_to_face, zbuf, dists, P, K, 1.0f / sigma, far, grad_zbuf, grad_dists);
+    B200R_LAUNCHED("soft_depth_backward_kernel");
+    return B200R_OK;
+  }
+  return launch_depth_warp_kernel<true>(grad_out, pix_to_face, zbuf, dists, P, K, 1.0f / sigma, far, nullptr,
+                                        grad_zbuf, grad_dists, stream);
+}
+
+extern "C" int b200r_hard_depth_forward(const int64_t* pix_to_face, const float* zbuf, int32_t N, int32_t H, int32_t W,
+                                        int32_t K, const float* zfar, float zfar_value, float* out, void* stream_) {
+  const int rc = depth_args(N, H, W, K);
+  if (rc != B200R_OK) return rc;
+  const int64_t P = (int64_t)N * H * W;
+  if (P == 0) return B200R_OK;
+  hard_depth_forward_kernel<<<(unsigned)blend_blocks(P, 0, 0), 256, 0, static_cast<cudaStream_t>(stream_)>>>(
+      pix_to_face, zbuf, P, K, DepthFar{zfar, zfar_value}, out);
+  B200R_LAUNCHED("hard_depth_forward_kernel");
+  return B200R_OK;
+}
+
+extern "C" int b200r_hard_depth_backward(const float* grad_out, const int64_t* pix_to_face, int32_t N, int32_t H,
+                                         int32_t W, int32_t K, float* grad_zbuf, void* stream_) {
+  const int rc = depth_args(N, H, W, K);
+  if (rc != B200R_OK) return rc;
+  const int64_t P = (int64_t)N * H * W;
+  if (P == 0) return B200R_OK;
+  hard_depth_backward_kernel<<<(unsigned)blend_blocks(P * K, 0, 0), 256, 0, static_cast<cudaStream_t>(stream_)>>>(
+      grad_out, pix_to_face, P, K, grad_zbuf);
+  B200R_LAUNCHED("hard_depth_backward_kernel");
+  return B200R_OK;
 }

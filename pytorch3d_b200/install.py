@@ -88,8 +88,19 @@ It replaces the three names in `pytorch3d.loss` and in their defining modules by
 `verts_packed()` is float32 CUDA and `faces_packed()` int64 CUDA on the same device, within the kernels' size limits
 (V < 2^31 - 1, 6F < 2^31), to `pytorch3d_b200.regularizers`; everything else (CPU tensors, float64 verts, oversized
 meshes, an unknown Laplacian method, for which the original raises) goes to the originals.
+
+`install_depth_shading()` (separate again) serves the depth shaders of depth-supervised fitting:
+    pytorch3d/renderer/mesh/shader.py       SoftDepthShader.forward, HardDepthShader.forward (pure torch)
+It replaces the method `forward` on both classes, as `install_textures()` does.  A call goes to
+`pytorch3d_b200.blending.soft_depth` / `hard_depth` when pix_to_face is int64 CUDA, zbuf (and dists for
+SoftDepthShader) float32 of the same 4-D shape on its device, 1 <= K <= 150, `blend_params.sigma` a real number, and
+zfar -- `kwargs.get("zfar", getattr(cameras, "zfar", 100.0))`, as the shaders resolve it -- a real number or a
+1-element float32 tensor on that device that does not require grad.  Everything else goes to the original method:
+CPU tensors, other dtypes, K = 0 or K > 150, `dists` None (for which SoftDepthShader raises), a per-image zfar of N > 1
+values (for which both raise), and a zfar that requires grad.
 """
 import importlib
+import numbers
 import types
 
 import torch
@@ -117,11 +128,14 @@ _NORMALS_OPS = ("face_areas_normals_forward", "face_areas_normals_backward")
 _MESHES_MODULE = "pytorch3d.structures.meshes"
 _LOSS_PACKAGE = "pytorch3d.loss"
 _LOSS_FUNCTIONS = ("mesh_edge_loss", "mesh_laplacian_smoothing", "mesh_normal_consistency")
+_SHADER_MODULE = "pytorch3d.renderer.mesh.shader"
+_DEPTH_SHADERS = ("SoftDepthShader", "HardDepthShader")
 _saved = {}
 # (module name, attribute) -> original (install_blending, install_splatter, install_shading, install_gouraud,
 # install_clipping and install_normals)
 _saved_blend = {}
-# (module name, class name, method name) -> original (install_textures, install_texture_atlas, install_normals)
+# (module name, class name, method name) -> original (install_textures, install_texture_atlas, install_normals,
+# install_depth_shading)
 _saved_methods = {}
 
 
@@ -614,10 +628,70 @@ def install_regularizers():
     return patched
 
 
+def _depth_fragments_fused(fragments, soft):
+    """int64 CUDA pix_to_face (N, H, W, K) with 1 <= K <= 150, and float32 zbuf (and dists) of its shape on its device."""
+    p2f = getattr(fragments, "pix_to_face", None)
+    if not (getattr(p2f, "is_cuda", False) and p2f.dtype == torch.int64 and p2f.dim() == 4
+            and 1 <= p2f.shape[3] <= _b200_C.kMaxPointsPerPixel):
+        return False
+    for name in ("zbuf", "dists") if soft else ("zbuf",):
+        t = getattr(fragments, name, None)
+        if not (getattr(t, "dtype", None) == torch.float32 and t.device == p2f.device and t.shape == p2f.shape):
+            return False
+    return True
+
+
+def _real(x):
+    return isinstance(x, numbers.Real) and not torch.is_tensor(x)
+
+
+def _zfar_fused(zfar, device):
+    """A real number, or a 1-element float32 tensor (0-d or (1,)) on `device` that does not require grad."""
+    if torch.is_tensor(zfar):
+        return (zfar.dtype == torch.float32 and zfar.numel() == 1 and zfar.dim() <= 1 and zfar.device == device
+                and not zfar.requires_grad)
+    return _real(zfar)
+
+
+def _depth_shader_dispatch(cls, original):
+    from . import blending as ours
+    soft = cls.__name__ == "SoftDepthShader"
+
+    def forward(self, fragments, meshes, **kwargs):
+        if _depth_fragments_fused(fragments, soft):
+            cameras = super(cls, self)._get_cameras(**kwargs)  # the reference's error when there are none
+            zfar = kwargs.get("zfar", getattr(cameras, "zfar", 100.0))
+            if _zfar_fused(zfar, fragments.pix_to_face.device):
+                if not soft:
+                    return ours.hard_depth(fragments, zfar)
+                sigma = self.blend_params.sigma
+                if _real(sigma):
+                    return ours.soft_depth(fragments, sigma, zfar)
+        return original(self, fragments, meshes, **kwargs)
+
+    forward.__qualname__ = cls.__name__ + ".forward"
+    forward.__doc__ = original.__doc__
+    return forward
+
+
+def install_depth_shading():
+    """Patch PyTorch3D's depth shaders (must be importable): the method `forward` of the classes `SoftDepthShader` and
+    `HardDepthShader` in pytorch3d.renderer.mesh.shader, so that existing shaders and every import path see it.
+    Returns the list of patched module names."""
+    m = importlib.import_module(_SHADER_MODULE)
+    for clsname in _DEPTH_SHADERS:
+        key = (_SHADER_MODULE, clsname, "forward")
+        if key not in _saved_methods:
+            cls = getattr(m, clsname)
+            _saved_methods[key] = cls.__dict__["forward"]
+            cls.forward = _depth_shader_dispatch(cls, cls.__dict__["forward"])
+    return [_SHADER_MODULE]
+
+
 def uninstall():
     """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_gouraud()`,
-    `install_textures()`, `install_texture_atlas()`, `install_clipping()`, `install_normals()` and
-    `install_regularizers()`."""
+    `install_textures()`, `install_texture_atlas()`, `install_clipping()`, `install_normals()`,
+    `install_regularizers()` and `install_depth_shading()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
