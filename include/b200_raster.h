@@ -478,6 +478,39 @@ int b200r_verts_normals_backward(const float* grad_normals, const float* verts, 
                                  size_t workspace_bytes, float* grad_verts, void* stream);
 
 /*
+ * Mesh surface sampling (DESIGN.md section 20): what pytorch3d.ops.sample_points_from_meshes computes, with draws from
+ * a counter-based generator.  verts float32 (V,3), faces int64 (F,3) packed, mesh_first_face / mesh_num_faces int64
+ * (N,), all contiguous device arrays read in place (64-bit offsets).  N >= 1, S >= 1, V < 2^31 - 1, N * S <= 2^40; the
+ * backward also needs 3 N S < 2^31.  All entry points are asynchronous, use no float atomics and are deterministic.
+ *
+ * forward: S samples per mesh, each face drawn with probability proportional to its face_areas_normals area (a face of
+ *  zero area never), barycentrics w0 = 1 - sqrt(u), w1 = sqrt(u) (1 - v), w2 = sqrt(u) v.  Writes samples (N,S,3),
+ *  normals (N,S,3) if not NULL ((v1 - v0) x (v2 - v1) normalised), face_idx (N,S) int64 (the packed face, -1 for a
+ *  mesh without faces, whose samples, normals and bary are zeros) and bary (N,S,3).  The draws come from one
+ *  Philox4x32-10 evaluation per sample, keyed by seed (2 int64 on the device, their low 32 bits) with the sample's
+ *  index n * S + s as counter; or, when draw_face, draw_u and draw_v ((N,S) int64 packed faces, float32 u and v) are
+ *  given, from those (seed may then be NULL).  *status (device int32) is set to the B200R_SAMPLE_* bits below.
+ * backward: grad_samples (N,S,3), grad_normals (N,S,3) or NULL, contiguous float32, with the forward's face_idx and
+ *  bary -> grad_verts (V,3).
+ * workspace: b200r_sample_points_workspace_bytes(V, F, N, S, pass) bytes, pass 0 for the forward and 1 for the
+ *  backward, a function of the shapes only (0 for bad sizes, or when there is no device to size the sort for).
+ */
+#define B200R_SAMPLE_HAS_VALID 1  /* some mesh has a face */
+#define B200R_SAMPLE_NONFINITE 2  /* some vertex coordinate is NaN or infinite */
+#define B200R_SAMPLE_BAD_TOTAL 4  /* a mesh with faces has a total area that is not positive and finite */
+#define B200R_SAMPLE_HAS_EMPTY 8  /* some mesh has no face */
+size_t b200r_sample_points_workspace_bytes(int64_t V, int64_t F, int64_t N, int64_t S, int32_t pass);
+int b200r_sample_points_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F,
+                                const int64_t* mesh_first_face, const int64_t* mesh_num_faces, int64_t N, int64_t S,
+                                const int64_t* seed, const int64_t* draw_face, const float* draw_u,
+                                const float* draw_v, void* workspace, size_t workspace_bytes, float* samples,
+                                float* normals, int64_t* face_idx, float* bary, int32_t* status, void* stream);
+int b200r_sample_points_backward(const float* grad_samples, const float* grad_normals, const float* verts, int64_t V,
+                                 const int64_t* faces, int64_t F, int64_t N, int64_t S, const int64_t* face_idx,
+                                 const float* bary, void* workspace, size_t workspace_bytes, float* grad_verts,
+                                 void* stream);
+
+/*
  * Mesh regularisers (DESIGN.md section 18): what pytorch3d/loss/mesh_edge_loss.py, mesh_laplacian_smoothing.py and
  * mesh_normal_consistency.py compute, as a float32 scalar `loss` (a device pointer), and its gradient to the verts.
  *  verts float32 (V,3) and faces int64 (F,3), contiguous, read in place (64-bit offsets); V < 2^31 - 1 and 6F < 2^31,

@@ -1177,6 +1177,142 @@ def verts_normals_backward(grad_normals: torch.Tensor, verts: torch.Tensor, face
     return grad_verts
 
 
+# Bits of the status word of sample_points_forward (B200R_SAMPLE_*).
+SAMPLE_HAS_VALID, SAMPLE_NONFINITE, SAMPLE_BAD_TOTAL, SAMPLE_HAS_EMPTY = 1, 2, 4, 8
+
+
+def _check_sampling_inputs(op, verts, faces, mesh_first_face, mesh_num_faces, num_samples):
+    """(V, F, N, S, device) of float32 verts (V, 3), int64 faces (F, 3) and the int64 (N,) per-mesh face ranges, all on
+    one CUDA device, N >= 1 and S >= 1; raises RuntimeError otherwise and for sizes past the kernels' limits."""
+    dev = _require_cuda(("verts", verts), ("faces", faces), ("mesh_first_face", mesh_first_face),
+                        ("mesh_num_faces", mesh_num_faces))
+    if verts.dtype != torch.float32:
+        raise RuntimeError("%s: expected scalar type Float for verts but found %s" % (op, verts.dtype))
+    if faces.dtype != torch.int64:
+        raise RuntimeError("%s: expected scalar type Long for faces but found %s" % (op, faces.dtype))
+    if verts.dim() != 2 or verts.shape[1] != 3:
+        raise RuntimeError("%s: verts must be (V, 3), got %s" % (op, tuple(verts.shape)))
+    if faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError("%s: faces must be (F, 3), got %s" % (op, tuple(faces.shape)))
+    N = int(mesh_first_face.shape[0]) if mesh_first_face.dim() == 1 else -1
+    for name, t in (("mesh_first_face", mesh_first_face), ("mesh_num_faces", mesh_num_faces)):
+        if t.dtype != torch.int64 or t.dim() != 1 or t.shape[0] != N or N < 1:
+            raise RuntimeError("%s: %s must be an int64 (N,) tensor with N >= 1 like mesh_first_face, got %s %s"
+                               % (op, name, t.dtype, tuple(t.shape)))
+    V, F, S = int(verts.shape[0]), int(faces.shape[0]), int(num_samples)
+    if S < 1:
+        raise RuntimeError("%s: num_samples must be at least 1, got %d" % (op, S))
+    if not sampling_sizes_ok(V, F, N, S):
+        raise RuntimeError("%s: at most 2^31 - 2 vertices, 2^31 - 1 meshes and 2^40 samples, got V = %d, F = %d, "
+                           "N = %d, S = %d" % (op, V, F, N, S))
+    return V, F, N, S, dev
+
+
+def sampling_sizes_ok(V: int, F: int, N: int, S: int):
+    """Whether the sampling kernels take these sizes (b200r_sample_points_forward)."""
+    return V < (1 << 31) - 1 and 1 <= N < (1 << 31) and F // 4096 + N + 1 < (1 << 31) and 1 <= S <= (1 << 40) // N
+
+
+def _sampling_workspace(lib, V, F, N, S, pass_, dev):
+    ws_bytes = int(lib.b200r_sample_points_workspace_bytes(V, F, N, S, pass_))
+    if ws_bytes == 0:
+        raise RuntimeError("sample_points: could not size the workspace (V = %d, F = %d, N = %d, S = %d)" % (V, F, N, S))
+    return torch.empty((ws_bytes,), dtype=torch.uint8, device=dev), ws_bytes  # 512-byte aligned
+
+
+def sample_points_forward(verts: torch.Tensor, faces: torch.Tensor, mesh_first_face: torch.Tensor,
+                          mesh_num_faces: torch.Tensor, num_samples: int, return_normals: bool, seed: torch.Tensor):
+    """Fused pytorch3d.ops.sample_points_from_meshes (DESIGN.md section 20): verts (V,3) f32, faces (F,3) i64 packed,
+    the per-mesh face ranges (N,) i64 and a seed, two int64 on the device (their low 32 bits key the generator) ->
+    (samples (N,S,3) f32, normals (N,S,3) f32 or None, face_idx (N,S) i64, bary (N,S,3) f32, status (1,) i32).  The
+    status bits (SAMPLE_*) are on the device; nothing here synchronises the host."""
+    return _sample_points(verts, faces, mesh_first_face, mesh_num_faces, num_samples, return_normals, seed, None)
+
+
+def _sample_points_from_draws(verts: torch.Tensor, faces: torch.Tensor, mesh_first_face: torch.Tensor,
+                              mesh_num_faces: torch.Tensor, return_normals: bool, face_idx: torch.Tensor,
+                              u: torch.Tensor, v: torch.Tensor):
+    """Test hook: `sample_points_forward` with the draws given -- face_idx (N,S) i64 packed faces, u and v (N,S) f32 --
+    instead of drawn, so that the outputs can be compared bit for bit with the reference's for the same draws."""
+    if face_idx.dim() != 2:
+        raise RuntimeError("face_idx must be (N, S), got %s" % (tuple(face_idx.shape),))
+    N, S = int(face_idx.shape[0]), int(face_idx.shape[1])
+    for name, t, dt in (("face_idx", face_idx, torch.int64), ("u", u, torch.float32), ("v", v, torch.float32)):
+        _require_cuda((name, t))
+        if t.dtype != dt or tuple(t.shape) != (N, S) or t.device != verts.device:
+            raise RuntimeError("%s must be a %s (N, S) tensor on %s" % (name, dt, verts.device))
+    draws = (face_idx.contiguous(), u.contiguous(), v.contiguous())
+    return _sample_points(verts, faces, mesh_first_face, mesh_num_faces, S, return_normals, None, draws)
+
+
+def _sample_points(verts, faces, mesh_first_face, mesh_num_faces, num_samples, return_normals, seed, draws):
+    V, F, N, S, dev = _check_sampling_inputs("sample_points_forward", verts, faces, mesh_first_face, mesh_num_faces,
+                                             num_samples)
+    if draws is None:
+        _require_cuda(("seed", seed))
+        if seed.dtype != torch.int64 or seed.numel() != 2 or seed.device != dev:
+            raise RuntimeError("seed must be two int64 on %s" % dev)
+        seed = seed.contiguous()
+    lib = _lib.load()
+    v, f = verts.contiguous(), faces.contiguous()
+    first, num = mesh_first_face.contiguous(), mesh_num_faces.contiguous()
+    with torch.cuda.device(dev):
+        samples = torch.empty((N, S, 3), dtype=torch.float32, device=dev)
+        normals = torch.empty((N, S, 3), dtype=torch.float32, device=dev) if return_normals else None
+        face_idx = torch.empty((N, S), dtype=torch.int64, device=dev)
+        bary = torch.empty((N, S, 3), dtype=torch.float32, device=dev)
+        status = torch.empty((1,), dtype=torch.int32, device=dev)
+        ws, ws_bytes = _sampling_workspace(lib, V, F, N, S, 0, dev)
+        d_face, d_u, d_v = draws if draws is not None else (None, None, None)
+        _lib.check(lib.b200r_sample_points_forward(
+            _ptr(v), V, _ptr(f), F, _ptr(first), _ptr(num), N, S, None if seed is None else seed.data_ptr(),
+            _ptr(d_face), _ptr(d_u), _ptr(d_v), ws.data_ptr(), ws_bytes, samples.data_ptr(), _ptr(normals),
+            face_idx.data_ptr(), bary.data_ptr(), status.data_ptr(), _stream_ptr(dev)))
+    return samples, normals, face_idx, bary, status
+
+
+def sample_points_backward(grad_samples: torch.Tensor, grad_normals, verts: torch.Tensor, faces: torch.Tensor,
+                           face_idx: torch.Tensor, bary: torch.Tensor):
+    """Backward of `sample_points_forward` -> grad_verts (V,3) f32, from the forward's face_idx and bary; grad_normals
+    may be None.  Deterministic, no float atomics, no host synchronisation."""
+    if face_idx.dim() != 2:
+        raise RuntimeError("face_idx must be (N, S), got %s" % (tuple(face_idx.shape),))
+    N, S = int(face_idx.shape[0]), int(face_idx.shape[1])
+    V, F, dev = _check_mesh_inputs_loose("sample_points_backward", verts, faces)
+    if 3 * N * S >= (1 << 31):
+        raise RuntimeError("sample_points_backward: the backward takes 3 N S < 2^31 sample corners, got N = %d, S = %d"
+                           % (N, S))
+    gs = _check_grad("grad_samples", grad_samples, (N, S, 3), dev)
+    gn = _check_grad("grad_normals", grad_normals, (N, S, 3), dev) if grad_normals is not None else None
+    b = _check_grad("bary", bary, (N, S, 3), dev)
+    _require_cuda(("face_idx", face_idx))
+    if face_idx.dtype != torch.int64 or face_idx.device != dev:
+        raise RuntimeError("face_idx must be the int64 (N, S) face_idx of sample_points_forward on %s" % dev)
+    lib = _lib.load()
+    v, f, fi = verts.contiguous(), faces.contiguous(), face_idx.contiguous()
+    with torch.cuda.device(dev):
+        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        ws, ws_bytes = _sampling_workspace(lib, V, F, N, S, 1, dev)
+        _lib.check(lib.b200r_sample_points_backward(_ptr(gs), _ptr(gn), _ptr(v), V, _ptr(f), F, N, S, _ptr(fi),
+                                                    _ptr(b), ws.data_ptr(), ws_bytes, _ptr(grad_verts),
+                                                    _stream_ptr(dev)))
+    return grad_verts
+
+
+def _check_mesh_inputs_loose(op, verts, faces):
+    """(V, F, device) of float32 verts (V, 3) and int64 faces (F, 3) on one CUDA device, V < 2^31 - 1."""
+    dev = _require_cuda(("verts", verts), ("faces", faces))
+    if verts.dtype != torch.float32 or verts.dim() != 2 or verts.shape[1] != 3:
+        raise RuntimeError("%s: verts must be a float32 (V, 3) tensor, got %s %s" % (op, verts.dtype,
+                                                                                      tuple(verts.shape)))
+    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError("%s: faces must be an int64 (F, 3) tensor, got %s %s" % (op, faces.dtype,
+                                                                                    tuple(faces.shape)))
+    if verts.shape[0] >= (1 << 31) - 1:
+        raise RuntimeError("%s: at most 2^31 - 2 vertices, got %d" % (op, verts.shape[0]))
+    return int(verts.shape[0]), int(faces.shape[0]), dev
+
+
 LAPLACIAN_METHODS = {"uniform": 0, "cot": 1, "cotcurv": 2}  # B200R_LAPLACIAN_*
 
 

@@ -109,6 +109,12 @@ SIGNATURES = {
     "b200r_face_areas_normals_backward": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
     "b200r_verts_normals_forward": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp, _vp, _vp]),
     "b200r_verts_normals_backward": (ctypes.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "b200r_sample_points_workspace_bytes": (_sz, [_i64, _i64, _i64, _i64, _i32]),
+    "b200r_sample_points_forward": (
+        ctypes.c_int,
+        [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200r_sample_points_backward": (
+        ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _sz, _vp, _vp]),
     "b200r_regularizers_workspace_bytes": (_sz, [_i64, _i64, _i32]),
     "b200r_mesh_edge_table": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _i32, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
     "b200r_mesh_edge_loss_forward": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i32, _f32, _vp, _sz, _vp, _vp]),

@@ -1,5 +1,6 @@
-// Mesh topology tables shared by the normals (normals.cu, DESIGN.md section 17) and the mesh regularisers
-// (regularizers.cu, section 18): the vertex -> corner table and the one segmented sum over it.
+// Mesh topology tables shared by the normals (normals.cu, DESIGN.md section 17), the mesh regularisers
+// (regularizers.cu, section 18) and the surface sampler (sampling.cu, section 20): the vertex -> corner table, the one
+// segmented sum over it, and the face-area and normalisation arithmetic they have in common.
 //
 // Corner j of face f has the id c = j * F + f and the key faces[f, j]; a stable radix sort of the 3F (key, id) pairs
 // over key_bits(V) bits, and an offset array of V + 1 entries, give every vertex the run of its corners in (j, f)
@@ -43,6 +44,38 @@ __device__ __forceinline__ float3 cross_fma(float3 a, float3 b) {
 // |s| as torch's 2-norm over dim 1 of a float32 (V, 3) tensor computes it.
 __device__ __forceinline__ float norm3(float3 s) {
   return __fsqrt_rn(__fmaf_rn(s.z, s.z, __fmaf_rn(s.y, s.y, __fmul_rn(s.x, s.x))));
+}
+
+__device__ __forceinline__ float3 sub_rn(float3 a, float3 b) {
+  return make_float3(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z));
+}
+
+// The cross product c = (p1 - p0) x (p2 - p0) and its norm as FaceAreasNormalsForwardKernel<float>
+// (pytorch3d/csrc/face_areas_normals/face_areas_normals.cu) is compiled by nvcc for sm_90a: each cross component is
+// FFMA(first product, -FMUL(second product)), the squared norm FFMA(cz, cz, FFMA(cx, cx, FMUL(cy, cy))), then an
+// IEEE square root.  The face's area is FMUL(norm, 0.5) (the reference's norm / 2.0 formed in double and rounded to
+// float is exactly that).  Shared by the face-area op (normals.cu) and the sampler (sampling.cu).
+__device__ __forceinline__ float face_cross_norm(const float3 p[3], float3& c) {
+  const float3 a = sub_rn(p[1], p[0]), b = sub_rn(p[2], p[0]);
+  c.x = __fmaf_rn(a.y, b.z, -__fmul_rn(a.z, b.y));
+  c.y = __fmaf_rn(a.z, b.x, -__fmul_rn(a.x, b.z));
+  c.z = __fmaf_rn(a.x, b.y, -__fmul_rn(a.y, b.x));
+  return __fsqrt_rn(__fmaf_rn(c.z, c.z, __fmaf_rn(c.x, c.x, __fmul_rn(c.y, c.y))));
+}
+
+// d loss / d s for y = s / clamp_min(|s|, eps), as autograd forms it: the quotient's two gradients, clamp_min's
+// (none below eps), and the norm's (none where |s| = 0).
+__device__ __forceinline__ float3 normalize_backward(float3 s, float3 g, float eps) {
+  const float n = norm3(s);
+  const float m = n < eps ? eps : n;
+  // div's gradient to the divisor, -g * ((s / m) / m), summed over the three components by expand_as's backward
+  const float gm = __fadd_rn(__fadd_rn(-__fmul_rn(g.x, __fdiv_rn(__fdiv_rn(s.x, m), m)),
+                                       -__fmul_rn(g.y, __fdiv_rn(__fdiv_rn(s.y, m), m))),
+                             -__fmul_rn(g.z, __fdiv_rn(__fdiv_rn(s.z, m), m)));
+  const float gn = n >= eps ? gm : 0.0f;               // clamp_min(norm, eps): where(norm >= eps, grad, 0)
+  const float k = n == 0.0f ? 0.0f : __fdiv_rn(gn, n);  // the norm's backward: s * (grad / norm), 0 where norm == 0
+  return make_float3(__fadd_rn(__fdiv_rn(g.x, m), __fmul_rn(s.x, k)), __fadd_rn(__fdiv_rn(g.y, m), __fmul_rn(s.y, k)),
+                     __fadd_rn(__fdiv_rn(g.z, m), __fmul_rn(s.z, k)));
 }
 
 __device__ __forceinline__ float3 load3(const float* __restrict__ p, int64_t i) {

@@ -27,10 +27,6 @@ namespace {
 
 constexpr size_t kAlign = 256;
 
-__device__ __forceinline__ float3 sub_rn(float3 a, float3 b) {
-  return make_float3(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z));
-}
-
 // ---- vertex normals -----------------------------------------------------------------------------------------------
 
 __global__ void __launch_bounds__(kThreads)
@@ -44,26 +40,13 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 
-// d loss / d s for y = s / clamp_min(|s|, eps), as autograd forms it: the quotient's two gradients, clamp_min's
-// (none below eps), and the norm's (none where |s| = 0).
+// d loss / d s for y = s / clamp_min(|s|, 1e-6) (mesh_tables.cuh normalize_backward).
 __global__ void __launch_bounds__(kThreads)
     normalize_backward_kernel(const float* __restrict__ grad_normals, const float* __restrict__ sums, int64_t V,
                               float* __restrict__ grad_sums) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < V; v += stride) {
-    const float3 s = load3(sums, v), g = load3(grad_normals, v);
-    const float n = norm3(s);
-    const float m = n < kNormalizeEps ? kNormalizeEps : n;
-    // div's gradient to the divisor, -g * ((s / m) / m), summed over the three components by expand_as's backward
-    const float gm = __fadd_rn(__fadd_rn(-__fmul_rn(g.x, __fdiv_rn(__fdiv_rn(s.x, m), m)),
-                                         -__fmul_rn(g.y, __fdiv_rn(__fdiv_rn(s.y, m), m))),
-                               -__fmul_rn(g.z, __fdiv_rn(__fdiv_rn(s.z, m), m)));
-    const float gn = n >= kNormalizeEps ? gm : 0.0f;     // clamp_min(norm, eps): where(norm >= eps, grad, 0)
-    const float k = n == 0.0f ? 0.0f : __fdiv_rn(gn, n);  // the norm's backward: s * (grad / norm), 0 where norm == 0
-    store3(grad_sums, v,
-           make_float3(__fadd_rn(__fdiv_rn(g.x, m), __fmul_rn(s.x, k)), __fadd_rn(__fdiv_rn(g.y, m), __fmul_rn(s.y, k)),
-                       __fadd_rn(__fdiv_rn(g.z, m), __fmul_rn(s.z, k))));
-  }
+  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < V; v += stride)
+    store3(grad_sums, v, normalize_backward(load3(sums, v), load3(grad_normals, v), kNormalizeEps));
 }
 
 // Per face: the gradient of n_f (the sum of grad_sums over its three corners), through the cross product and the two
@@ -94,25 +77,20 @@ __global__ void __launch_bounds__(kThreads)
 
 // ---- face areas and normals ---------------------------------------------------------------------------------------
 
-// FaceAreasNormalsForwardKernel<float> as nvcc compiles it for sm_90a: each cross component is FFMA(first product,
-// -FMUL(second product)), the squared norm FFMA(cz, cz, FFMA(cx, cx, FMUL(cy, cy))), then an IEEE square root.  The
-// area norm / 2.0, formed in double and rounded to float, is exactly FMUL(norm, 0.5).  The clamp compares in double
-// (NaN passes) and clamps to (float)1e-6; the normal is an IEEE divide.
+// FaceAreasNormalsForwardKernel<float> as nvcc compiles it for sm_90a: the cross product, norm and area of
+// face_cross_norm (mesh_tables.cuh).  The clamp compares in double (NaN passes) and clamps to (float)1e-6; the normal is
+// an IEEE divide.
 __global__ void __launch_bounds__(kThreads)
     face_areas_normals_forward_kernel(const float* __restrict__ verts, const int64_t* __restrict__ faces, int64_t V,
                                       int64_t F, float* __restrict__ areas, float* __restrict__ normals) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += stride) {
-    float3 p[3];
+    float3 p[3], c;
     face_corners(verts, faces, V, f, p);
-    const float3 a = sub_rn(p[1], p[0]), b = sub_rn(p[2], p[0]);
-    const float cx = __fmaf_rn(a.y, b.z, -__fmul_rn(a.z, b.y));
-    const float cy = __fmaf_rn(a.z, b.x, -__fmul_rn(a.x, b.z));
-    const float cz = __fmaf_rn(a.x, b.y, -__fmul_rn(a.y, b.x));
-    float norm = __fsqrt_rn(__fmaf_rn(cz, cz, __fmaf_rn(cx, cx, __fmul_rn(cy, cy))));
+    float norm = face_cross_norm(p, c);
     areas[f] = __fmul_rn(norm, 0.5f);
     norm = ((double)norm < 1e-6) ? (float)1e-6 : norm;
-    store3(normals, f, make_float3(__fdiv_rn(cx, norm), __fdiv_rn(cy, norm), __fdiv_rn(cz, norm)));
+    store3(normals, f, make_float3(__fdiv_rn(c.x, norm), __fdiv_rn(c.y, norm), __fdiv_rn(c.z, norm)));
   }
 }
 

@@ -98,6 +98,15 @@ zfar -- `kwargs.get("zfar", getattr(cameras, "zfar", 100.0))`, as the shaders re
 1-element float32 tensor on that device that does not require grad.  Everything else goes to the original method:
 CPU tensors, other dtypes, K = 0 or K > 150, `dists` None (for which SoftDepthShader raises), a per-image zfar of N > 1
 values (for which both raise), and a zfar that requires grad.
+
+`install_sampling()` (separate again) serves the surface sampling of the mesh-to-mesh fitting loop:
+    pytorch3d/ops/__init__.py                       from .sample_points_from_meshes import sample_points_from_meshes
+    pytorch3d/ops/sample_points_from_meshes.py      sample_points_from_meshes (torch: multinomial, rand, gathers)
+It replaces the function in its defining module and the name in `pytorch3d.ops` (where the import makes the package
+attribute the function, not the submodule) by one that sends meshes whose `verts_packed()` is float32 CUDA and
+`faces_packed()` int64 CUDA on the same device, with an integer num_samples >= 1, within the kernels' size limits, to
+`pytorch3d_b200.sampling`; everything else (CPU tensors, float64 verts, oversized inputs, and `return_textures=True`
+on a batch containing a mesh without faces, for which the original raises) goes to the original.
 """
 import importlib
 import numbers
@@ -128,11 +137,13 @@ _NORMALS_OPS = ("face_areas_normals_forward", "face_areas_normals_backward")
 _MESHES_MODULE = "pytorch3d.structures.meshes"
 _LOSS_PACKAGE = "pytorch3d.loss"
 _LOSS_FUNCTIONS = ("mesh_edge_loss", "mesh_laplacian_smoothing", "mesh_normal_consistency")
+_OPS_PACKAGE = "pytorch3d.ops"
+_SAMPLING_MODULE = "pytorch3d.ops.sample_points_from_meshes"
 _SHADER_MODULE = "pytorch3d.renderer.mesh.shader"
 _DEPTH_SHADERS = ("SoftDepthShader", "HardDepthShader")
 _saved = {}
 # (module name, attribute) -> original (install_blending, install_splatter, install_shading, install_gouraud,
-# install_clipping and install_normals)
+# install_clipping, install_normals, install_regularizers and install_sampling)
 _saved_blend = {}
 # (module name, class name, method name) -> original (install_textures, install_texture_atlas, install_normals,
 # install_depth_shading)
@@ -628,6 +639,46 @@ def install_regularizers():
     return patched
 
 
+def _sampling_fused(meshes, num_samples):
+    """Whether the fused sampler takes this call: at least one mesh, float32 CUDA verts and int64 CUDA faces on one
+    device, an integer num_samples >= 1, within the kernels' size limits."""
+    if len(meshes) == 0 or not isinstance(num_samples, numbers.Integral) or isinstance(num_samples, bool):
+        return False
+    verts, faces = meshes.verts_packed(), meshes.faces_packed()
+    return _mesh_fused(verts, faces) and _b200_C.sampling_sizes_ok(int(verts.shape[0]), int(faces.shape[0]),
+                                                                   len(meshes), int(num_samples))
+
+
+def _sampling_dispatch(original):
+    from . import sampling as ours
+
+    def sample_points_from_meshes(meshes, num_samples: int = 10000, return_normals: bool = False,
+                                  return_textures: bool = False):
+        if _sampling_fused(meshes, num_samples):
+            try:
+                return ours.sample_points_from_meshes(meshes, num_samples, return_normals, return_textures)
+            except ours.EmptyMeshWithTextures:
+                pass
+        return original(meshes, num_samples, return_normals, return_textures)
+
+    sample_points_from_meshes.__doc__ = original.__doc__
+    return sample_points_from_meshes
+
+
+def install_sampling():
+    """Patch PyTorch3D's surface sampling (must be importable): `sample_points_from_meshes` in
+    pytorch3d.ops.sample_points_from_meshes and in pytorch3d.ops.  Returns the list of patched module names."""
+    package = importlib.import_module(_OPS_PACKAGE)
+    module = importlib.import_module(_SAMPLING_MODULE)
+    name = "sample_points_from_meshes"
+    original = module.__dict__[name]
+    for owner, key in ((module, _SAMPLING_MODULE), (package, _OPS_PACKAGE)):
+        if (key, name) not in _saved_blend:
+            _saved_blend[(key, name)] = owner.__dict__[name]
+            setattr(owner, name, _sampling_dispatch(original))
+    return [_OPS_PACKAGE, _SAMPLING_MODULE]
+
+
 def _depth_fragments_fused(fragments, soft):
     """int64 CUDA pix_to_face (N, H, W, K) with 1 <= K <= 150, and float32 zbuf (and dists) of its shape on its device."""
     p2f = getattr(fragments, "pix_to_face", None)
@@ -691,7 +742,7 @@ def install_depth_shading():
 def uninstall():
     """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_gouraud()`,
     `install_textures()`, `install_texture_atlas()`, `install_clipping()`, `install_normals()`,
-    `install_regularizers()` and `install_depth_shading()`."""
+    `install_regularizers()`, `install_depth_shading()` and `install_sampling()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
