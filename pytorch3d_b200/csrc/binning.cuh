@@ -53,7 +53,6 @@ __device__ __forceinline__ bool rect_empty(uint2 r) { return (r.x & 0xFFFFu) > (
 
 // The tile counters are zeroed by a kernel the setup pass is chained to (programmatic dependent launch) instead of a memset
 // node: the setup pass's loads and arithmetic overlap it and wait only before their first atomic (binning -1.8 us).
-#ifndef B200R_EXP_MEMSET_NODE
 static __global__ void __launch_bounds__(256) zero_ints_kernel(int* __restrict__ p, int64_t n) {
   const int64_t i = ((int64_t)blockIdx.x * 256 + threadIdx.x) * 4;
   pdl_trigger();
@@ -62,7 +61,6 @@ static __global__ void __launch_bounds__(256) zero_ints_kernel(int* __restrict__
   else
     for (int64_t j = i; j < n && j < i + 4; ++j) p[j] = 0;
 }
-#endif
 
 // Count one element per tile of its rectangle.  Called by ALL 32 lanes of a warp (lanes without work pass an
 // empty rectangle): consecutive elements of a packed mesh are neighbours on screen, so most lanes of a warp
@@ -120,7 +118,10 @@ __device__ __forceinline__ void warp_count_rect(uint2 r, int n, int TY, int TX, 
 // blur-band tile of the north-star batch runs for ~120 us of a 920 us kernel).  Keeping the raster order inside a class
 // keeps neighbouring tiles -- which share most of their faces' records -- in flight together (an arbitrary order inside
 // the classes cost config 5 11 %).  Three classes: longer than the mean non-empty list, shorter, empty; the per-class
-// ranks of all tiles come from ONE block scan of a packed counter (3 x 21 bits).
+// ranks of all tiles come from ONE block scan of a packed counter (3 x 21 bits).  (Without a blur band, placing the
+// covered tiles evenly among the empty ones by these ranks -- a merge of (r + 1/2) / covered and (s + 1/2) / empty --
+// ran the north-star fine pass in 210.9 us, no faster than the fixed row stride of FineParams::row_stride (210.1 us),
+// and this pass's second sweep took the binning from 64.6 to 74.7 us; H100 SXM, 700 W.)
 #ifdef B200R_EXP_ORDER4  // (experiment: four classes -- > 2 x mean, > mean, shorter, empty -- of 16-bit counters)
 constexpr int ORDER_BITS = 16, ORDER_CLASSES = 4;
 __device__ __forceinline__ int order_class(int count, int mean) {

@@ -13,6 +13,7 @@
 // The K nearest hits are the reference's queue: keys in registers, payload in shared memory.
 #include <cfloat>
 #include <climits>
+#include <numeric>
 
 #include "binning.cuh"
 #include "bulk_copy.cuh"
@@ -480,7 +481,8 @@ struct FineParams {
   const int64_t* first;
   const int64_t* num;
   const int* tile_offset;
-  const int* tile_order;  // schedule: the CTA with linear index b takes tile tile_order[b] (nullptr: tile b)
+  const int* tile_order;  // schedule: the CTA with linear index b takes tile tile_order[b] (nullptr: see row_stride)
+  int row_stride;  // without tile_order: CTA row y takes tile row (y * row_stride) mod TY (coprime with TY)
   int* pairs;  // tile lists; each CTA puts its own segment in ascending face order before reading it
   int64_t capacity;
   int n0;  // first image of this launch (grid.z is limited to 65535 images)
@@ -580,6 +582,33 @@ __device__ __forceinline__ void store_pair_run(float4* run, const float4 (&mine)
     const float4 vo = 2 * j + 1 < P ? recv[2 * j + 1 < P ? j : 0] : mine[2 * j + 1 >= P ? 2 * j + 1 - P : 0];
     const bool target_a = odd ? (2 * j + 1 < P) : (2 * j < P);
     if (target_a ? vA : vB) out_store(run + 2 * j + odd, odd ? vo : ve);
+  }
+}
+
+// The same with the pieces made on demand: `piece(i)` returns this lane's piece i.  For even P the exchange falls
+// apart into P / 2 independent rounds -- round r swaps piece 2r (odd lane) for piece 2r+1 (even lane) and writes run
+// pieces 2r, 2r+1 (first pixel) and P+2r, P+2r+1 (second pixel), each instruction whole sectors -- so only two pieces
+// of a lane are live at a time instead of all P (the K = 8 barycentrics: 6 pieces, the epilogue's register peak).
+template <int P, class PieceFn>
+__device__ __forceinline__ void store_pair_pieces(float4* run, PieceFn piece, int odd, bool vA, bool vB) {
+  if constexpr (P % 2 == 0) {
+#pragma unroll
+    for (int r = 0; r < P / 2; ++r) {
+      const float4 a = piece(2 * r), b = piece(2 * r + 1);
+      const float4 send = odd ? a : b;
+      float4 recv;
+      recv.x = __shfl_xor_sync(0xffffffffu, send.x, 1);
+      recv.y = __shfl_xor_sync(0xffffffffu, send.y, 1);
+      recv.z = __shfl_xor_sync(0xffffffffu, send.z, 1);
+      recv.w = __shfl_xor_sync(0xffffffffu, send.w, 1);
+      if (vA) out_store(run + 2 * r + odd, odd ? recv : a);
+      if (vB) out_store(run + P + 2 * r + odd, odd ? b : recv);
+    }
+  } else {
+    float4 mine[P];
+#pragma unroll
+    for (int i = 0; i < P; ++i) mine[i] = piece(i);
+    store_pair_run<P>(run, mine, odd, vA, vB);
   }
 }
 
@@ -978,17 +1007,18 @@ struct TileWork {
 __device__ __forceinline__ TileWork tile_work(const FineParams& p) {
   pdl_wait();  // the tile lists (fill kernel) and, transitively, the face records are complete (see common.cuh)
   TileWork t;
-  int i = ((p.n0 + blockIdx.z) * p.TY + blockIdx.y) * p.TX + blockIdx.x;  // linear index of this CTA
+  int i;
   if (p.tile_order != nullptr) {
-    i = p.tile_order[i];  // heavy tiles first, empty tiles last (see tile_scan_kernel)
+    i = p.tile_order[((p.n0 + blockIdx.z) * p.TY + blockIdx.y) * p.TX + blockIdx.x];  // (see tile_scan_kernel)
     t.tile_x = i % p.TX;
     const int r = i / p.TX;
     t.tile_y = r % p.TY;
     t.n = r / p.TY;
   } else {
     t.tile_x = blockIdx.x;
-    t.tile_y = blockIdx.y;
+    t.tile_y = (int)((blockIdx.y * (unsigned)p.row_stride) % (unsigned)p.TY);  // (see row_stride)
     t.n = p.n0 + blockIdx.z;
+    i = (t.n * p.TY + t.tile_y) * p.TX + t.tile_x;
   }
   // the tile's face list; tiles whose segment did not fit the pair buffer test every face of the mesh
   t.seg_begin = p.tile_offset[i];
@@ -1020,7 +1050,8 @@ __device__ __forceinline__ int first_walk_order(const FineParams& p, const TileW
 
 // Resident CTAs per SM the fine kernels are compiled for (__launch_bounds__ minBlocks: the register cap is
 // 65536 / (FTHREADS * CTAS)).  On sm_90a the scan-conversion path (no blur) spills at 64 registers: with 3 CTAs per SM
-// (80 registers) the north-star fine pass takes 222 us instead of 254 us, and the K = 16 shared-memory-queue pass with 2
+// (80 registers) the north-star fine pass takes 222 us instead of 254 us (with the epilogue of store_pair_pieces it
+// still spills 160 B at 64 registers, 24 B at 80), and the K = 16 shared-memory-queue pass with 2
 // instead of 3 CTAs 395 us instead of 407 us; the blur path is faster at 4 CTAs (891 us against 944 us at 3).
 // (H100 80GB HBM3 SXM, 700 W power limit, tools/variant_time.py.)
 #ifndef B200R_FINE_CTAS
@@ -1044,7 +1075,9 @@ __global__ void __launch_bounds__(FTHREADS, SCAN ? B200R_FINE_SCAN_CTAS : B200R_
   const TileWork t = tile_work(p);
   const int tile_x = t.tile_x, tile_y = t.tile_y, n = t.n;
   if (t.count == 0) {
+#ifndef B200R_EXP_COVERED_ONLY  // (timing experiment: covered tiles alone)
     write_empty_tile<KMAX>(p, n, tile_x, tile_y);
+#endif
     return;
   }
   int xo, yo;
@@ -1090,51 +1123,37 @@ __global__ void __launch_bounds__(FTHREADS, SCAN ? B200R_FINE_SCAN_CTAS : B200R_
     const bool vA = __shfl_sync(0xffffffffu, (int)valid, lane & ~1) != 0;
     const bool vB = __shfl_sync(0xffffffffu, (int)valid, lane | 1) != 0;
     const int64_t oa = o - (int64_t)odd * KMAX;  // the even lane's pixel
-    {
-      // pix_to_face: int64, but the values are the queue's int32 face ids: exchange those, widen at the store
-      float4 piece[KMAX / 2];
+    // (pieces are made as they are stored, see store_pair_pieces: the slot loops below unroll to constant indices)
+    // pix_to_face: int64, but the values are the queue's int32 face ids: exchange those, widen at the store
+    store_pair_pieces<KMAX / 2>(reinterpret_cast<float4*>(p.pix_to_face + oa), [&](int i) {
+      const long long i0 = 2 * i >= q.size ? -1ll : (long long)q.id[2 * i];
+      const long long i1 = 2 * i + 1 >= q.size ? -1ll : (long long)q.id[2 * i + 1];
+      return make_float4(__int_as_float((int)(i0 & 0xffffffffll)), __int_as_float((int)(i0 >> 32)),
+                         __int_as_float((int)(i1 & 0xffffffffll)), __int_as_float((int)(i1 >> 32)));
+    }, odd, vA, vB);
+    store_pair_pieces<KMAX / 4>(reinterpret_cast<float4*>(p.zbuf + oa), [&](int i) {
+      const int k0 = 4 * i;
+      return make_float4(k0 + 0 >= q.size ? -1.0f : q.z[k0 + 0], k0 + 1 >= q.size ? -1.0f : q.z[k0 + 1],
+                         k0 + 2 >= q.size ? -1.0f : q.z[k0 + 2], k0 + 3 >= q.size ? -1.0f : q.z[k0 + 3]);
+    }, odd, vA, vB);
+    store_pair_pieces<KMAX / 4>(reinterpret_cast<float4*>(p.dists + oa), [&](int i) {
+      float d[4];
 #pragma unroll
-      for (int k = 0; k < KMAX; k += 2) {
-        const long long i0 = k >= q.size ? -1ll : (long long)q.id[k];
-        const long long i1 = k + 1 >= q.size ? -1ll : (long long)q.id[k + 1];
-        piece[k / 2] = make_float4(__int_as_float((int)(i0 & 0xffffffffll)), __int_as_float((int)(i0 >> 32)),
-                                   __int_as_float((int)(i1 & 0xffffffffll)), __int_as_float((int)(i1 >> 32)));
+      for (int u = 0; u < 4; ++u) d[u] = 4 * i + u >= q.size ? -1.0f : pay[slot[4 * i + u] * FTHREADS].x;
+      return make_float4(d[0], d[1], d[2], d[3]);
+    }, odd, vA, vB);
+    // barycentrics: piece 3m + c holds words 4c .. 4c+3 of the twelve (b0, b1, b2) words of slots 4m .. 4m+3
+    store_pair_pieces<3 * KMAX / 4>(reinterpret_cast<float4*>(p.bary + oa * 3), [&](int i) {
+      const int k0 = 4 * (i / 3), c = i % 3;
+      float4 w[2];  // the two slots the piece draws from
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const int k = k0 + c + u;
+        w[u] = k >= q.size ? make_float4(-1.f, -1.f, -1.f, -1.f) : pay[slot[k] * FTHREADS];
       }
-      store_pair_run<KMAX / 2>(reinterpret_cast<float4*>(p.pix_to_face + oa), piece, odd, vA, vB);
-    }
-    {
-      float4 piece[KMAX / 4];
-#pragma unroll
-      for (int k0 = 0; k0 < KMAX; k0 += 4)
-        piece[k0 / 4] = make_float4(k0 + 0 >= q.size ? -1.0f : q.z[k0 + 0], k0 + 1 >= q.size ? -1.0f : q.z[k0 + 1],
-                                    k0 + 2 >= q.size ? -1.0f : q.z[k0 + 2], k0 + 3 >= q.size ? -1.0f : q.z[k0 + 3]);
-      store_pair_run<KMAX / 4>(reinterpret_cast<float4*>(p.zbuf + oa), piece, odd, vA, vB);
-    }
-    {
-      float4 piece[KMAX / 4];
-#pragma unroll
-      for (int k0 = 0; k0 < KMAX; k0 += 4) {
-        float d[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) d[u] = k0 + u >= q.size ? -1.0f : pay[slot[k0 + u] * FTHREADS].x;
-        piece[k0 / 4] = make_float4(d[0], d[1], d[2], d[3]);
-      }
-      store_pair_run<KMAX / 4>(reinterpret_cast<float4*>(p.dists + oa), piece, odd, vA, vB);
-    }
-    {
-      float4 piece[3 * KMAX / 4];
-#pragma unroll
-      for (int k0 = 0; k0 < KMAX; k0 += 4) {
-        float4 w[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-          w[u] = k0 + u >= q.size ? make_float4(-1.f, -1.f, -1.f, -1.f) : pay[slot[k0 + u] * FTHREADS];
-        piece[3 * (k0 / 4) + 0] = make_float4(w[0].y, w[0].z, w[0].w, w[1].y);
-        piece[3 * (k0 / 4) + 1] = make_float4(w[1].z, w[1].w, w[2].y, w[2].z);
-        piece[3 * (k0 / 4) + 2] = make_float4(w[2].w, w[3].y, w[3].z, w[3].w);
-      }
-      store_pair_run<3 * KMAX / 4>(reinterpret_cast<float4*>(p.bary + oa * 3), piece, odd, vA, vB);
-    }
+      return c == 0 ? make_float4(w[0].y, w[0].z, w[0].w, w[1].y)
+                    : (c == 1 ? make_float4(w[0].z, w[0].w, w[1].y, w[1].z) : make_float4(w[0].w, w[1].y, w[1].z, w[1].w));
+    }, odd, vA, vB);
     stored = true;
    }
   }
@@ -1663,6 +1682,7 @@ __global__ void __launch_bounds__(TILE_THREADS, PF ? B200R_BWD_PF_CTAS : B200R_B
   const bool persp = p.persp != 0, clip = p.clip != 0;
   constexpr int G = GV > 0 ? GV : 1;
   static_assert(!PF || GV == 8, "the prefetching variant is the K % 8 == 0 kernel");
+  pdl_wait();  // the gradient is zeroed by the kernel this one is chained to (see zero_gradient)
 
   for (int k0 = 0; k0 < K; k0 += G) {
     int fk[G];
@@ -1809,7 +1829,8 @@ static int forward_impl(const float* face_verts, const float* verts, int64_t V, 
   }
   // Schedule of the fine pass (see tile_scan_kernel): worth the extra pass of the scan kernel and one more dependent load
   // per CTA where tiles run long -- with a blur band (north-star batch + blur 1e-4: fine 918 -> 749 us, config 2: 137 ->
-  // 109 us); without one the north-star batch loses 6 us.  The packed class counters hold 2^21 tiles.
+  // 109 us); without one the north-star batch loses 6 us.  The packed class counters hold 2^21 tiles.  Without a blur
+  // band the fine pass instead takes its tile rows in a fixed stride (see row_stride below).
 #ifdef B200R_EXP_NOTILEORDER
   int* const tile_order = nullptr;
 #else
@@ -1834,6 +1855,18 @@ static int forward_impl(const float* face_verts, const float* verts, int64_t V, 
   p.num = num;
   p.tile_offset = ws.tile_offset;
   p.tile_order = tile_order;
+  // Without a blur band a tile either is empty (a pure store stream of its -1 fill) or runs a short compute phase
+  // before its stores; in raster order the covered tiles sit together in the middle rows of each image, so waves of
+  // CTAs alternate between HBM-bound and compute-bound.  Taking the rows at a stride of ~0.38 TY (coprime with TY)
+  // mixes both kinds into every wave while a row's tiles stay adjacent: north-star fine pass 215.6 -> 210.1 us, K = 16
+  // 394.7 -> 379.6 us (H100 SXM, 700 W; tools/time_fine_floor.py, tools/variant_time.py).
+  p.row_stride = 1;
+#ifndef B200R_EXP_RASTER_ROWS  // (timing experiment: raster order)
+  if (!(blur_radius > 0.0f)) {
+    p.row_stride = (int)(TY * 0.382) | 1;
+    while (std::gcd(p.row_stride, TY) != 1) p.row_stride += 2;
+  }
+#endif
   p.pairs = ws.pairs;
   p.capacity = ws.capacity;
   p.N = N; p.H = H; p.W = W; p.K = K; p.TY = TY; p.TX = TX;
@@ -1944,6 +1977,15 @@ extern "C" int b200r_rasterize_meshes_forward_indexed(const float* verts, int64_
                       zbuf, bary, dists, workspace, workspace_bytes, pair_capacity, stream_);
 }
 
+// The backward pass accumulates into its gradient output, which a kernel zeroes first -- a normal launch, after the
+// forward pass has completed -- and the backward kernel is chained to it, so that its CTAs are resident when the zeroing
+// drains.  (Measured: the zeroing kernel chained to the fine pass as well, with the fine kernels triggering at their
+// top, took the north-star step from 0.4154 to 0.4117 ms but config 2's from 0.2226 to 0.2305 ms; H100 SXM, 700 W.)
+static cudaError_t zero_gradient(float* g, int64_t n, cudaStream_t stream) {
+  zero_ints_kernel<<<(unsigned)((n + 1023) / 1024), 256, 0, stream>>>(reinterpret_cast<int*>(g), n);
+  return cudaGetLastError();
+}
+
 static int backward_impl(const float* face_verts, int64_t F, const int64_t* pix_to_face, const float* grad_zbuf,
                          const float* grad_bary, const float* grad_dists, int32_t N, int32_t H, int32_t W, int32_t K,
                          int32_t perspective_correct, int32_t clip_barycentric_coords, float* grad_face_verts,
@@ -1951,7 +1993,7 @@ static int backward_impl(const float* face_verts, int64_t F, const int64_t* pix_
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (F < 0 || N < 0 || H < 0 || W < 0 || K < 0) return fail(B200R_ERR_INVALID_ARGUMENT, "negative size");
   if (F == 0) return B200R_OK;
-  if (faces == nullptr) B200R_CUDA_OK(cudaMemsetAsync(grad_face_verts, 0, sizeof(float) * 9 * (size_t)F, stream));
+  if (faces == nullptr) B200R_CUDA_OK(zero_gradient(grad_face_verts, 9 * F, stream));
   if ((int64_t)N * H * W * K == 0) return B200R_OK;
   const int TY = div_up(H, TILE), TX = div_up(W, TILE);
   BackwardParams p;
@@ -1978,13 +2020,13 @@ static int backward_impl(const float* face_verts, int64_t F, const int64_t* pix_
     const bool prefetch = false && aligned;
 #endif
     if ((K & 7) == 0 && prefetch)
-      mesh_backward_kernel<8, true><<<bgrid, TILE_THREADS, 0, stream>>>(p);
+      B200R_CUDA_OK(launch_chained((mesh_backward_kernel<8, true>), bgrid, dim3(TILE_THREADS), 0, stream, p));
     else if ((K & 7) == 0)
-      mesh_backward_kernel<8, false><<<bgrid, TILE_THREADS, 0, stream>>>(p);
+      B200R_CUDA_OK(launch_chained((mesh_backward_kernel<8, false>), bgrid, dim3(TILE_THREADS), 0, stream, p));
     else if ((K & 3) == 0)
-      mesh_backward_kernel<4, false><<<bgrid, TILE_THREADS, 0, stream>>>(p);
+      B200R_CUDA_OK(launch_chained((mesh_backward_kernel<4, false>), bgrid, dim3(TILE_THREADS), 0, stream, p));
     else
-      mesh_backward_kernel<0, false><<<bgrid, TILE_THREADS, 0, stream>>>(p);
+      B200R_CUDA_OK(launch_chained((mesh_backward_kernel<0, false>), bgrid, dim3(TILE_THREADS), 0, stream, p));
   }
   B200R_LAUNCHED("mesh_backward_kernel");
   if (prof) {
@@ -2012,7 +2054,7 @@ extern "C" int b200r_rasterize_meshes_backward_indexed(const float* face_verts, 
                                                        float* grad_face_verts_scratch, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (F < 0 || V < 0) return fail(B200R_ERR_INVALID_ARGUMENT, "negative size");
-  if (V > 0) B200R_CUDA_OK(cudaMemsetAsync(grad_verts, 0, sizeof(float) * 3 * (size_t)V, stream));
+  if (V > 0) B200R_CUDA_OK(zero_gradient(grad_verts, 3 * V, stream));
   if (F == 0 || V == 0) return B200R_OK;
   // (the kernel adds every group's gradient straight to the three vertices of its face: no (F,3,3) intermediate and
   // no scatter pass -- 20 MB written and read again and one launch less per step at the north-star size;
