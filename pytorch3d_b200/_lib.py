@@ -33,17 +33,13 @@ SIGNATURES = {
         [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _i32, _i32, _i32, _i32,
          _vp, _vp, _vp, _vp, _vp, _vp, _sz, _i64, _vp]),
     "b200r_rasterize_meshes_backward_indexed": (
-        ctypes.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+        ctypes.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "b200r_rasterize_points_workspace_bytes": (_sz, [_i64, _i32, _i32, _i32, _i64]),
     "b200r_rasterize_points_forward": (
         ctypes.c_int,
         [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _i64, _vp]),
     "b200r_rasterize_points_backward": (
         ctypes.c_int, [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
-    "b200r_alpha_composite_forward": (
-        ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
-    "b200r_alpha_composite_backward": (
-        ctypes.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "b200r_alpha_composite_forward_strided": (
         ctypes.c_int, [_vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
     "b200r_alpha_composite_backward_strided": (

@@ -87,7 +87,6 @@ __device__ __forceinline__ void warp_count_rect(uint2 r, int n, int TY, int TX, 
   for (int i = 0; i < rounds; ++i) {
     const bool act = i < ntile;
     const int t = act ? (n * TY + ty) * TX + tx : -1 - lane;  // inactive lanes get unique keys
-#ifndef B200R_EXP_AGG_MATCH
     // runs of consecutive lanes with the same tile -- a shuffle and two votes -- instead of __match_any_sync, whose result
     // the atomic waited for (17 % of the setup kernel's stall samples; north-star binning 44.7 -> 40.8 us, config 2 23.6 ->
     // 21.5 us); equal tiles that are not adjacent in the warp cost one more atomic
@@ -98,10 +97,6 @@ __device__ __forceinline__ void warp_count_rect(uint2 r, int n, int TY, int TX, 
       const unsigned after = lane == 31 ? 0u : conts >> (lane + 1);
       atomicAdd(tile_count + t, 1 + (__ffs((int)~after) - 1));
     }
-#else
-    const unsigned grp = __match_any_sync(0xffffffffu, t);
-    if (act && lane == __ffs(grp) - 1) atomicAdd(tile_count + t, __popc(grp));
-#endif
     if (++tx > tx1) {
       tx = tx0;
       ++ty;
@@ -122,15 +117,8 @@ __device__ __forceinline__ void warp_count_rect(uint2 r, int n, int TY, int TX, 
 // covered tiles evenly among the empty ones by these ranks -- a merge of (r + 1/2) / covered and (s + 1/2) / empty --
 // ran the north-star fine pass in 210.9 us, no faster than the fixed row stride of FineParams::row_stride (210.1 us),
 // and this pass's second sweep took the binning from 64.6 to 74.7 us; H100 SXM, 700 W.)
-#ifdef B200R_EXP_ORDER4  // (experiment: four classes -- > 2 x mean, > mean, shorter, empty -- of 16-bit counters)
-constexpr int ORDER_BITS = 16, ORDER_CLASSES = 4;
-__device__ __forceinline__ int order_class(int count, int mean) {
-  return count <= 0 ? 3 : (count > 2 * mean ? 0 : (count > mean ? 1 : 2));
-}
-#else
 constexpr int ORDER_BITS = 21, ORDER_CLASSES = 3;
 __device__ __forceinline__ int order_class(int count, int mean) { return count <= 0 ? 2 : (count > mean ? 0 : 1); }
-#endif
 __device__ __forceinline__ unsigned long long order_key(int count, int mean) {
   return 1ull << (ORDER_BITS * order_class(count, mean));
 }
@@ -330,7 +318,6 @@ static __global__ void __launch_bounds__(256)
   for (int i = 0; i < rounds; ++i) {
     const bool act = i < ntile;
     const int t = act ? (n * TY + ty) * TX + tx : -1 - lane;
-#ifndef B200R_EXP_AGG_MATCH
     const int tprev = __shfl_up_sync(0xffffffffu, t, 1);
     const bool cont = act && lane > 0 && t == tprev;
     const unsigned conts = __ballot_sync(0xffffffffu, cont);
@@ -345,15 +332,6 @@ static __global__ void __launch_bounds__(256)
     base = __shfl_sync(0xffffffffu, base, leader);
     if (act) {
       const int pos = base + (lane - leader);
-#else
-    const unsigned grp = __match_any_sync(0xffffffffu, t);
-    const int leader = __ffs(grp) - 1;
-    int base = 0;
-    if (act && lane == leader) base = atomicAdd(cursor + t, __popc(grp));
-    base = __shfl_sync(0xffffffffu, base, leader);
-    if (act) {
-      const int pos = base + __popc(grp & ((1u << lane) - 1u));
-#endif
       if (pos >= 0 && (int64_t)pos < capacity) pairs[pos] = (int)e;  // (pos < 0: saturated / wrapped cursor)
     }
     if (++tx > tx1) {
@@ -407,12 +385,6 @@ static __global__ void __launch_bounds__(256)
       for (int tx = tx0; tx <= tx1; ++tx) atomicAdd(hist + ty * TX + tx, 1);
   }
   __syncthreads();
-#ifdef B200R_EXP_PFILL_SERIAL
-  for (int t = tid; t < T; t += 256) {
-    const int c = hist[t];
-    if (c > 0) hist[t] = atomicAdd(cursor + n0 * T + t, c);  // start of this CTA's range in the tile's segment
-  }
-#else
   // (four returning atomics in flight per thread: each would wait for its own round trip to L2 otherwise)
   for (int t0 = tid; t0 < T; t0 += 4 * 256) {
     int c[4], b[4];
@@ -424,7 +396,6 @@ static __global__ void __launch_bounds__(256)
     for (int u = 0; u < 4; ++u)
       if (c[u] > 0) hist[t0 + u * 256] = b[u];  // start of this CTA's range in the tile's segment
   }
-#endif
   __syncthreads();
 #pragma unroll
   for (int i = 0; i < BIN_CHUNK / 256; ++i) {
@@ -561,43 +532,6 @@ __device__ __forceinline__ void cta_sort_segment(int* seg, int n, int* s_keys, i
   }
   if (in_smem)
     for (int i = threadIdx.x; i < n; i += NT) seg[i] = s_keys[i];
-  __syncthreads();
-}
-
-// A tile list of any length put in ascending order of 64-bit keys built by `make_key(element)`; the keys live in shared
-// memory (`keys`, room for n of them), the list itself is rewritten in that order.  Used by the mesh fine pass to walk a
-// tile's faces front to back (key = (nearest vertex depth, face)).
-template <int NT, class MakeKey>
-__device__ __forceinline__ void cta_sort_segment_by_key(int* seg, int n, unsigned long long* keys, MakeKey make_key) {
-  for (int i = threadIdx.x; i < n; i += NT) keys[i] = make_key(seg[i]);
-  __syncthreads();
-  for (int k = 2; (k >> 1) < n; k <<= 1) {
-    for (int i = threadIdx.x; i < n; i += NT) {  // mirror step
-      const int j = i ^ (k - 1);
-      if (j > i && j < n) {
-        const unsigned long long a = keys[i], b = keys[j];
-        if (b < a) {
-          keys[i] = b;
-          keys[j] = a;
-        }
-      }
-    }
-    __syncthreads();
-    for (int d = k >> 2; d > 0; d >>= 1) {
-      for (int i = threadIdx.x; i < n; i += NT) {
-        const int j = i ^ d;
-        if (j > i && j < n) {
-          const unsigned long long a = keys[i], b = keys[j];
-          if (b < a) {
-            keys[i] = b;
-            keys[j] = a;
-          }
-        }
-      }
-      __syncthreads();
-    }
-  }
-  for (int i = threadIdx.x; i < n; i += NT) seg[i] = (int)(unsigned)(keys[i] & 0xffffffffull);
   __syncthreads();
 }
 

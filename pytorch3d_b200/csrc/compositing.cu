@@ -485,14 +485,6 @@ static int check_comp_args(int64_t C, int64_t P, int32_t N, int32_t K, int32_t H
   return B200R_OK;
 }
 
-extern "C" int b200r_alpha_composite_forward(const float* features, int64_t C, int64_t P, const float* alphas,
-                                             const int64_t* alpha_strides, const int64_t* points_idx,
-                                             const int64_t* idx_strides, int32_t N, int32_t K, int32_t H, int32_t W,
-                                             float* result, void* stream_) {
-  return b200r_alpha_composite_forward_strided(features, C, P, P, 1, alphas, alpha_strides, points_idx, idx_strides, N,
-                                               K, H, W, result, stream_);
-}
-
 extern "C" int b200r_alpha_composite_forward_strided(const float* features, int64_t C, int64_t P,
                                                      int64_t feature_stride_c, int64_t feature_stride_p,
                                                      const float* alphas, const int64_t* alpha_strides,
@@ -519,15 +511,6 @@ extern "C" int b200r_alpha_composite_forward_strided(const float* features, int6
 #undef B200R_AC_FWD
   B200R_LAUNCHED("alpha_composite_forward_kernel");
   return B200R_OK;
-}
-
-extern "C" int b200r_alpha_composite_backward(const float* grad_out, const float* features, int64_t C, int64_t P,
-                                              const float* alphas, const int64_t* alpha_strides,
-                                              const int64_t* points_idx, const int64_t* idx_strides, int32_t N,
-                                              int32_t K, int32_t H, int32_t W, float* grad_features,
-                                              float* grad_alphas, void* stream_) {
-  return b200r_alpha_composite_backward_strided(grad_out, features, C, P, P, 1, alphas, alpha_strides, points_idx,
-                                                idx_strides, N, K, H, W, grad_features, grad_alphas, stream_);
 }
 
 extern "C" int b200r_alpha_composite_backward_strided(const float* grad_out, const float* features, int64_t C,

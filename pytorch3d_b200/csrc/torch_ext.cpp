@@ -197,7 +197,7 @@ at::Tensor rasterize_meshes_backward_indexed(const at::Tensor& face_verts, const
   check_status(b200r_rasterize_meshes_backward_indexed(
       f32_or_null(fv), i64_or_null(faces), F, V, i64_or_null(p2f), f32_or_null(gz), f32_or_null(gb), f32_or_null(gd),
       (int32_t)p2f.size(0), (int32_t)p2f.size(1), (int32_t)p2f.size(2), (int32_t)p2f.size(3), perspective_correct,
-      clip_barycentric_coords, f32_or_null(grad_verts), nullptr, stream));
+      clip_barycentric_coords, f32_or_null(grad_verts), stream));
   return grad_verts;
 }
 
