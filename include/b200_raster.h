@@ -499,6 +499,51 @@ int b200r_sample_points_backward(const float* grad_samples, const float* grad_no
                                  void* stream);
 
 /*
+ * Chamfer distance (DESIGN.md section 21): what pytorch3d/loss/chamfer.py's chamfer_distance computes for D = 3, with
+ * the nearest neighbours of the reference's KNearestNeighborKernelV3<float, 3, 1> bit for bit.  x (N,P1,3) and y
+ * (N,P2,3) float32, x_lengths / y_lengths int64 (N,) or NULL (all P), x_normals (N,P1,3) and y_normals (N,P2,3) float32
+ * or both NULL, weights float32 (N,) or NULL, all contiguous device arrays.  N, P1, P2 >= 1 and 2 (N P1 + N P2) < 2^31.
+ * All entry points are asynchronous, use no float atomics and are deterministic.
+ *
+ * forward: dist_x / idx_x (N,P1) and, unless single_directional, dist_y / idx_y (N,P2): each point's nearest-neighbour
+ *  distance and index in the other cloud (0 and 0 for padding and for an empty other cloud).  cloud (4N + 1 floats)
+ *  and argmax (2N int32) keep the per-cloud state the backward reads.  Outputs: with point_reduction NONE, the distance
+ *  terms out_x (N,P1) and out_y (N,P2) and the normal terms out_nx / out_ny; otherwise the loss in out_x and the normal
+ *  loss in out_nx ((N,) for batch_reduction NONE, else one float).  *status (device int32) gets the B200R_CHAMFER_*
+ *  bits of the data-dependent checks below.
+ * backward: grad_x / grad_y (and grad_nx / grad_ny) are the upstream gradients of the outputs in the same layout
+ *  (grad_y and grad_ny only for point_reduction NONE) -> grad_points (N P1 + N P2, 3): x's rows, then y's; and
+ *  grad_normals likewise.  Either may be NULL.
+ * workspace: b200r_chamfer_workspace_bytes(N, P1, P2, pass) bytes, pass 0 for the forward and 1 for the backward.
+ */
+#define B200R_CHAMFER_POINT_NONE 0
+#define B200R_CHAMFER_POINT_SUM 1
+#define B200R_CHAMFER_POINT_MEAN 2
+#define B200R_CHAMFER_POINT_MAX 3
+#define B200R_CHAMFER_BATCH_NONE 0
+#define B200R_CHAMFER_BATCH_SUM 1
+#define B200R_CHAMFER_BATCH_MEAN 2
+#define B200R_CHAMFER_X_LENGTH 1      /* some x_lengths[n] > P1 */
+#define B200R_CHAMFER_Y_LENGTH 2      /* some y_lengths[n] > P2 */
+#define B200R_CHAMFER_W_NEGATIVE 4    /* some weight is not >= 0 */
+#define B200R_CHAMFER_W_ZERO_SUM 8    /* the weights sum to 0 */
+size_t b200r_chamfer_workspace_bytes(int64_t N, int64_t P1, int64_t P2, int32_t pass);
+int b200r_chamfer_forward(const float* x, const float* y, int64_t N, int64_t P1, int64_t P2, const int64_t* x_lengths,
+                          const int64_t* y_lengths, const float* x_normals, const float* y_normals,
+                          const float* weights, int32_t norm, int32_t point_reduction, int32_t batch_reduction,
+                          int32_t single_directional, int32_t abs_cosine, void* workspace, size_t workspace_bytes,
+                          float* dist_x, int32_t* idx_x, float* dist_y, int32_t* idx_y, float* cloud, int32_t* argmax,
+                          float* out_x, float* out_y, float* out_nx, float* out_ny, int32_t* status, void* stream);
+int b200r_chamfer_backward(const float* x, const float* y, int64_t N, int64_t P1, int64_t P2,
+                           const int64_t* x_lengths, const int64_t* y_lengths, const float* x_normals,
+                           const float* y_normals, const float* weights, int32_t norm, int32_t point_reduction,
+                           int32_t batch_reduction, int32_t single_directional, int32_t abs_cosine,
+                           const int32_t* idx_x, const int32_t* idx_y, const float* cloud, const int32_t* argmax,
+                           const float* grad_x, const float* grad_y, const float* grad_nx, const float* grad_ny,
+                           void* workspace, size_t workspace_bytes, float* grad_points, float* grad_normals,
+                           void* stream);
+
+/*
  * Mesh regularisers (DESIGN.md section 18): what pytorch3d/loss/mesh_edge_loss.py, mesh_laplacian_smoothing.py and
  * mesh_normal_consistency.py compute, as a float32 scalar `loss` (a device pointer), and its gradient to the verts.
  *  verts float32 (V,3) and faces int64 (F,3), contiguous, read in place (64-bit offsets); V < 2^31 - 1 and 6F < 2^31,

@@ -1313,6 +1313,152 @@ def _check_mesh_inputs_loose(op, verts, faces):
     return int(verts.shape[0]), int(faces.shape[0]), dev
 
 
+# Reductions and status bits of chamfer_forward (B200R_CHAMFER_*).
+CHAMFER_POINT = {None: 0, "sum": 1, "mean": 2, "max": 3}
+CHAMFER_BATCH = {None: 0, "sum": 1, "mean": 2}
+CHAMFER_X_LENGTH, CHAMFER_Y_LENGTH, CHAMFER_W_NEGATIVE, CHAMFER_W_ZERO_SUM = 1, 2, 4, 8
+
+
+def chamfer_sizes_ok(N: int, P1: int, P2: int):
+    """Whether the chamfer kernels take these sizes (b200r_chamfer_forward): the backward's sort ids are int32."""
+    return N >= 1 and P1 >= 1 and P2 >= 1 and 2 * (N * P1 + N * P2) < (1 << 31)
+
+
+def _chamfer_workspace(lib, N, P1, P2, pass_, dev):
+    ws_bytes = int(lib.b200r_chamfer_workspace_bytes(N, P1, P2, pass_))
+    if ws_bytes == 0:
+        raise RuntimeError("chamfer: could not size the workspace (N = %d, P1 = %d, P2 = %d)" % (N, P1, P2))
+    return torch.empty((ws_bytes,), dtype=torch.uint8, device=dev), ws_bytes
+
+
+def _check_chamfer_inputs(op, x, y, x_lengths, y_lengths, x_normals, y_normals, weights):
+    """(N, P1, P2, device): float32 x (N, P1, 3) and y (N, P2, 3), int64 (N,) lengths, float32 normals of the clouds'
+    shapes and float32 (N,) weights, all on one CUDA device; raises RuntimeError otherwise."""
+    named = [("x", x), ("y", y)] + [(k, t) for k, t in (("x_lengths", x_lengths), ("y_lengths", y_lengths),
+                                                        ("x_normals", x_normals), ("y_normals", y_normals),
+                                                        ("weights", weights)) if t is not None]
+    dev = _require_cuda(*named)
+    for name, t in named:
+        if t.device != dev:
+            raise RuntimeError("%s: expected all tensors on %s, %s is on %s" % (op, dev, name, t.device))
+    for name, t in (("x", x), ("y", y)):
+        if t.dtype != torch.float32 or t.dim() != 3 or t.shape[2] != 3:
+            raise RuntimeError("%s: %s must be a float32 (N, P, 3) tensor, got %s %s" % (op, name, t.dtype,
+                                                                                       tuple(t.shape)))
+    N, P1, P2 = int(x.shape[0]), int(x.shape[1]), int(y.shape[1])
+    if y.shape[0] != N:
+        raise RuntimeError("%s: x and y must have the same batch size" % op)
+    for name, t, P in (("x_lengths", x_lengths, P1), ("y_lengths", y_lengths, P2)):
+        if t is not None and (t.dtype != torch.int64 or tuple(t.shape) != (N,)):
+            raise RuntimeError("%s: %s must be an int64 (N,) tensor" % (op, name))
+    if (x_normals is None) != (y_normals is None):
+        raise RuntimeError("%s: give both normals or neither" % op)
+    for name, t, P in (("x_normals", x_normals, P1), ("y_normals", y_normals, P2)):
+        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != (N, P, 3)):
+            raise RuntimeError("%s: %s must be a float32 (%d, %d, 3) tensor" % (op, name, N, P))
+    if weights is not None and (weights.dtype != torch.float32 or tuple(weights.shape) != (N,)):
+        raise RuntimeError("%s: weights must be a float32 (N,) tensor" % op)
+    if not chamfer_sizes_ok(N, P1, P2):
+        raise RuntimeError("%s: takes N, P1, P2 >= 1 and 2 (N P1 + N P2) < 2^31, got N = %d, P1 = %d, P2 = %d"
+                           % (op, N, P1, P2))
+    return N, P1, P2, dev
+
+
+def _c(t):
+    return t.contiguous() if t is not None else None
+
+
+def chamfer_forward(x, y, x_lengths, y_lengths, x_normals, y_normals, weights, norm: int, point_reduction,
+                    batch_reduction, single_directional: bool, abs_cosine: bool):
+    """Fused pytorch3d.loss.chamfer_distance for D = 3 (DESIGN.md section 21).  Returns (outputs, state, status):
+    outputs (loss_x, loss_y, normals_x, normals_y) -- per-point terms for point_reduction None, else the loss and the
+    normal loss in the first and third (None where absent); state (dist_x, idx_x, dist_y, idx_y, cloud, argmax) for
+    the backward; status (1,) i32 with the CHAMFER_* bits on the device.  Nothing here synchronises the host."""
+    N, P1, P2, dev = _check_chamfer_inputs("chamfer_forward", x, y, x_lengths, y_lengths, x_normals, y_normals,
+                                           weights)
+    if norm not in (1, 2):
+        raise RuntimeError("chamfer_forward: norm must be 1 or 2")
+    pr, br = CHAMFER_POINT[point_reduction], CHAMFER_BATCH[batch_reduction]
+    if pr == 0 and br != 0:
+        raise RuntimeError("chamfer_forward: batch_reduction must be None when point_reduction is None")
+    lib = _lib.load()
+    x, y, xl, yl, xn, yn, w = (_c(t) for t in (x, y, x_lengths, y_lengths, x_normals, y_normals, weights))
+    nrm = xn is not None
+    f32 = dict(dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        dist_x = torch.empty((N, P1), **f32)
+        idx_x = torch.empty((N, P1), dtype=torch.int32, device=dev)
+        dist_y = torch.empty((N, P2), **f32) if not single_directional else None
+        idx_y = torch.empty((N, P2), dtype=torch.int32, device=dev) if not single_directional else None
+        cloud = torch.empty((4 * N + 1,), **f32)
+        argmax = torch.empty((2 * N,), dtype=torch.int32, device=dev)
+        status = torch.empty((1,), dtype=torch.int32, device=dev)
+        if pr == 0:
+            out_x = torch.empty((N, P1), **f32)
+            out_y = torch.empty((N, P2), **f32) if not single_directional else None
+            out_nx = torch.empty((N, P1), **f32) if nrm else None
+            out_ny = torch.empty((N, P2), **f32) if nrm and not single_directional else None
+        else:
+            shape = (N,) if br == 0 else ()
+            out_x, out_y = torch.empty(shape, **f32), None
+            out_nx, out_ny = (torch.empty(shape, **f32) if nrm else None), None
+        ws, ws_bytes = _chamfer_workspace(lib, N, P1, P2, 0, dev)
+        _lib.check(lib.b200r_chamfer_forward(
+            _ptr(x), _ptr(y), N, P1, P2, _ptr(xl), _ptr(yl), _ptr(xn), _ptr(yn), _ptr(w), int(norm), pr, br,
+            int(bool(single_directional)), int(bool(abs_cosine)), ws.data_ptr(), ws_bytes, _ptr(dist_x),
+            _ptr(idx_x), _ptr(dist_y), _ptr(idx_y), _ptr(cloud), _ptr(argmax), _ptr(out_x), _ptr(out_y),
+            _ptr(out_nx), _ptr(out_ny), _ptr(status), _stream_ptr(dev)))
+    return (out_x, out_y, out_nx, out_ny), (dist_x, idx_x, dist_y, idx_y, cloud, argmax), status
+
+
+def chamfer_backward(x, y, x_lengths, y_lengths, x_normals, y_normals, weights, norm: int, point_reduction,
+                     batch_reduction, single_directional: bool, abs_cosine: bool, state, grads, need_points: bool,
+                     need_normals: bool):
+    """Backward of `chamfer_forward`: grads (g_x, g_y, g_nx, g_ny) are the upstream gradients of its outputs (None
+    for an output without one: zeros) -> (grad_x, grad_y, grad_x_normals, grad_y_normals), the pairs asked for by
+    need_points / need_normals (None otherwise).  Deterministic, no float atomics, no host synchronisation."""
+    N, P1, P2, dev = _check_chamfer_inputs("chamfer_backward", x, y, x_lengths, y_lengths, x_normals, y_normals,
+                                           weights)
+    pr, br = CHAMFER_POINT[point_reduction], CHAMFER_BATCH[batch_reduction]
+    dist_x, idx_x, dist_y, idx_y, cloud, argmax = state
+    nrm = x_normals is not None
+    need_normals = need_normals and nrm
+    if not (need_points or need_normals):
+        return None, None, None, None
+    lib = _lib.load()
+    x, y, xl, yl, xn, yn, w = (_c(t) for t in (x, y, x_lengths, y_lengths, x_normals, y_normals, weights))
+    shapes = ((N, P1), (N, P2)) if pr == 0 else ((((N,) if br == 0 else ())),) * 2
+    g = []
+    for k, t in enumerate(grads):
+        present = (k % 2 == 0 or pr == 0) and (k < 2 or nrm) and not (k % 2 == 1 and single_directional)
+        if not present:
+            g.append(None)
+        elif t is None:
+            g.append(torch.zeros(shapes[k % 2], dtype=torch.float32, device=dev))
+        else:
+            g.append(t.to(torch.float32).contiguous())
+    with torch.cuda.device(dev):
+        V = N * P1 + N * P2
+        gp = torch.empty((V, 3), dtype=torch.float32, device=dev) if need_points else None
+        gn = torch.empty((V, 3), dtype=torch.float32, device=dev) if need_normals else None
+        ws, ws_bytes = _chamfer_workspace(lib, N, P1, P2, 1, dev)
+        _lib.check(lib.b200r_chamfer_backward(
+            _ptr(x), _ptr(y), N, P1, P2, _ptr(xl), _ptr(yl), _ptr(xn), _ptr(yn), _ptr(w), int(norm), pr, br,
+            int(bool(single_directional)), int(bool(abs_cosine)), _ptr(idx_x), _ptr(idx_y), _ptr(cloud),
+            _ptr(argmax), _ptr(g[0]), _ptr(g[1]), _ptr(g[2]), _ptr(g[3]), ws.data_ptr(), ws_bytes, _ptr(gp),
+            _ptr(gn), _stream_ptr(dev)))
+    gx, gy = (gp[:N * P1].view(N, P1, 3), gp[N * P1:].view(N, P2, 3)) if gp is not None else (None, None)
+    gnx, gny = (gn[:N * P1].view(N, P1, 3), gn[N * P1:].view(N, P2, 3)) if gn is not None else (None, None)
+    return gx, gy, gnx, gny
+
+
+def _chamfer_nn(x, y, x_lengths=None, y_lengths=None, norm: int = 2):
+    """Test hook: the fused search alone -- (dist_x (N,P1) f32, idx_x (N,P1) i64, dist_y (N,P2) f32, idx_y (N,P2)
+    i64), each point's nearest neighbour in the other cloud as the reference's knn_points(K=1) finds it."""
+    _, state, _ = chamfer_forward(x, y, x_lengths, y_lengths, None, None, None, norm, None, None, False, True)
+    return state[0], state[1].long(), state[2], state[3].long()
+
+
 LAPLACIAN_METHODS = {"uniform": 0, "cot": 1, "cotcurv": 2}  # B200R_LAPLACIAN_*
 
 

@@ -107,6 +107,15 @@ attribute the function, not the submodule) by one that sends meshes whose `verts
 `faces_packed()` int64 CUDA on the same device, with an integer num_samples >= 1, within the kernels' size limits, to
 `pytorch3d_b200.sampling`; everything else (CPU tensors, float64 verts, oversized inputs, and `return_textures=True`
 on a batch containing a mesh without faces, for which the original raises) goes to the original.
+
+`install_chamfer()` (separate again) serves the loss of both fitting loops:
+    pytorch3d/loss/__init__.py                      from .chamfer import chamfer_distance
+    pytorch3d/loss/chamfer.py                       chamfer_distance (knn_points, knn_gather, torch reductions)
+It replaces the function in its defining module and the name in `pytorch3d.loss` by one that sends float32 CUDA
+clouds with D = 3 on one device (tensors or Pointclouds), with int64 (N,) lengths, float32 (N, P, 3) normals and
+float32 (N,) weights that do not require grad on that device, within the kernels' size limits, to
+`pytorch3d_b200.chamfer`; everything else (CPU tensors, float64, D != 3, mixed devices, weights that require grad,
+oversized inputs, and calls the reference rejects) goes to the original.
 """
 import importlib
 import numbers
@@ -143,7 +152,7 @@ _SHADER_MODULE = "pytorch3d.renderer.mesh.shader"
 _DEPTH_SHADERS = ("SoftDepthShader", "HardDepthShader")
 _saved = {}
 # (module name, attribute) -> original (install_blending, install_splatter, install_shading, install_gouraud,
-# install_clipping, install_normals, install_regularizers and install_sampling)
+# install_clipping, install_normals, install_regularizers, install_sampling and install_chamfer)
 _saved_blend = {}
 # (module name, class name, method name) -> original (install_textures, install_texture_atlas, install_normals,
 # install_depth_shading)
@@ -679,6 +688,81 @@ def install_sampling():
     return [_OPS_PACKAGE, _SAMPLING_MODULE]
 
 
+_CHAMFER_MODULE = "pytorch3d.loss.chamfer"
+
+
+def _chamfer_cloud(points, lengths, normals):
+    """(points, lengths, normals) as chamfer.py reads them from a tensor or a Pointclouds-like object."""
+    if torch.is_tensor(points):
+        return points, lengths, normals
+    if hasattr(points, "points_padded") and hasattr(points, "num_points_per_cloud"):
+        return points.points_padded(), points.num_points_per_cloud(), points.normals_padded()
+    return None, None, None
+
+
+def _chamfer_fused(x, y, x_lengths, y_lengths, x_normals, y_normals, weights, norm, point_reduction):
+    """Whether the fused chamfer_distance takes this call: float32 CUDA (N, P, 3) clouds with D = 3 on one device,
+    int64 (N,) lengths and float32 (N, P, 3) normals there, float32 (N,) weights that do not require grad, within the
+    kernels' size limits.  Calls the reference rejects go to it too, so that it raises."""
+    x, x_lengths, x_normals = _chamfer_cloud(x, x_lengths, x_normals)
+    y, y_lengths, y_normals = _chamfer_cloud(y, y_lengths, y_normals)
+    if x is None or y is None or norm not in (1, 2) or isinstance(norm, bool):
+        return False
+    if point_reduction == "max" and (x_normals is not None or y_normals is not None):
+        return False
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.shape[2] == 3):
+        return False
+    dev = x.device
+    if not (y.is_cuda and y.device == dev and y.dtype == torch.float32 and y.dim() == 3 and y.shape[2] == 3
+            and y.shape[0] == x.shape[0]):
+        return False
+    N, P1, P2 = int(x.shape[0]), int(x.shape[1]), int(y.shape[1])
+    for t in (x_lengths, y_lengths):
+        if t is not None and not (torch.is_tensor(t) and t.is_cuda and t.device == dev and t.dtype == torch.int64
+                                  and tuple(t.shape) == (N,)):
+            return False
+    if x_normals is not None and y_normals is not None:
+        for t, P in ((x_normals, P1), (y_normals, P2)):
+            if not (torch.is_tensor(t) and t.is_cuda and t.device == dev and t.dtype == torch.float32
+                    and tuple(t.shape) == (N, P, 3)):
+                return False
+    if weights is not None and not (torch.is_tensor(weights) and weights.is_cuda and weights.device == dev
+                                    and weights.dtype == torch.float32 and tuple(weights.shape) == (N,)
+                                    and not weights.requires_grad):
+        return False
+    return _b200_C.chamfer_sizes_ok(N, P1, P2)
+
+
+def _chamfer_dispatch(original):
+    from . import chamfer as ours
+
+    def chamfer_distance(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_normals=None, weights=None,
+                         batch_reduction="mean", point_reduction="mean", norm: int = 2,
+                         single_directional: bool = False, abs_cosine: bool = True):
+        args = (x, y, x_lengths, y_lengths, x_normals, y_normals, weights, batch_reduction, point_reduction, norm,
+                single_directional, abs_cosine)
+        if _chamfer_fused(x, y, x_lengths, y_lengths, x_normals, y_normals, weights, norm, point_reduction):
+            return ours.chamfer_distance(*args)
+        return original(*args)
+
+    chamfer_distance.__doc__ = original.__doc__
+    return chamfer_distance
+
+
+def install_chamfer():
+    """Patch PyTorch3D's chamfer loss (must be importable): `chamfer_distance` in pytorch3d.loss.chamfer and in
+    pytorch3d.loss.  Returns the list of patched module names."""
+    package = importlib.import_module(_LOSS_PACKAGE)
+    module = importlib.import_module(_CHAMFER_MODULE)
+    name = "chamfer_distance"
+    original = module.__dict__[name]
+    for owner, key in ((module, _CHAMFER_MODULE), (package, _LOSS_PACKAGE)):
+        if (key, name) not in _saved_blend:
+            _saved_blend[(key, name)] = owner.__dict__[name]
+            setattr(owner, name, _chamfer_dispatch(original))
+    return [_LOSS_PACKAGE, _CHAMFER_MODULE]
+
+
 def _depth_fragments_fused(fragments, soft):
     """int64 CUDA pix_to_face (N, H, W, K) with 1 <= K <= 150, and float32 zbuf (and dists) of its shape on its device."""
     p2f = getattr(fragments, "pix_to_face", None)
@@ -742,7 +826,7 @@ def install_depth_shading():
 def uninstall():
     """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_gouraud()`,
     `install_textures()`, `install_texture_atlas()`, `install_clipping()`, `install_normals()`,
-    `install_regularizers()`, `install_depth_shading()` and `install_sampling()`."""
+    `install_regularizers()`, `install_depth_shading()`, `install_sampling()` and `install_chamfer()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
