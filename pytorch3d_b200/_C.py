@@ -176,104 +176,108 @@ def rasterize_points_backward(points: torch.Tensor, idxs: torch.Tensor, grad_zbu
     return _ext().rasterize_points_backward(points, idxs, grad_zbuf, grad_dists)
 
 
+
+# ------------------------------------------------------------------------------------------------ the ctypes ops
+# Every op below checks each tensor it hands the library by pointer (device, then dtype and shape, then the kernels'
+# size limits) and calls the library through `_launch`.
+
+F32, I32, I64 = torch.float32, torch.int32, torch.int64
+_TYPE_NAMES = {F32: "Float", I32: "Int", I64: "Long", torch.bool: "Bool"}
+
+
+def _launch(dev, name, *args):
+    """b200r_<name>(*args, current stream of dev) on the device `dev`; a failed status raises RuntimeError."""
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        _lib.check(getattr(lib, "b200r_" + name)(*args, _stream_ptr(dev)))
+
+
+def _workspace_size(name, *sizes):
+    return int(getattr(_lib.load(), "b200r_%s_workspace_bytes" % name)(*sizes))
+
+
+def _workspace(dev, name, *sizes, required=False):
+    """(uint8 workspace on dev, its bytes) as b200r_<name>_workspace_bytes(*sizes) sizes it; (None, 0) when it needs
+    none, unless `required`: then a size of 0 raises.  The caching allocator's blocks are 512-byte aligned."""
+    ws_bytes = _workspace_size(name, *sizes)
+    if ws_bytes == 0 and required:
+        raise RuntimeError("%s: could not size the workspace for sizes %s" % (name, sizes))
+    return (torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None), ws_bytes
+
+
+# The two dtype errors of ATen, which the reference's ops raise: data_ptr<T>()'s, here with the argument named at the
+# end, and checkScalarType's, which the blending, shading and texture ops use for their float inputs.
+_DATA_PTR_TEXT = "expected scalar type {want} but found {got} for {name}"
+_SCALAR_TYPE_TEXT = "Expected tensor for {name} to have scalar type {want}; but got {got}"
+
+
+def _check_tensor(name, t, dtype, shape=None, dims=None, op=None, text=_DATA_PTR_TEXT):
+    """Raises RuntimeError unless `t` has `dtype` and `shape`, each when given (None in `shape` leaves a dimension
+    free).  The message names the op when given, the argument, and the expected dtype (in `text`) or shape (`dims`,
+    default the sizes)."""
+    if dtype is not None and t.dtype != dtype:
+        raise RuntimeError((op + ": " if op else "") + text.format(want=_TYPE_NAMES[dtype], got=t.dtype, name=name))
+    if shape is not None and not _fits(t.shape, shape):
+        if dims is None:
+            dims = ", ".join("*" if s is None else str(s) for s in shape) + ("," if len(shape) == 1 else "")
+        raise RuntimeError("%s%s must be (%s), got %s" % (op + ": " if op else "", name, dims, tuple(t.shape)))
+
+
+def _check_float(name, t, shape=None, dims=None):
+    """_check_tensor for a float32 input of the blending, shading and texture ops, with checkScalarType's text."""
+    _check_tensor(name, t, F32, shape, dims, text=_SCALAR_TYPE_TEXT)
+
+
+def _fits(size, shape):
+    """Whether `size` is `shape`, where None leaves a dimension free."""
+    if len(size) != len(shape):
+        return False
+    for n, s in zip(size, shape):
+        if s is not None and s != n:
+            return False
+    return True
+
+
+def _check_verts_faces(op, verts, faces, *named):
+    """(V, F, device) of float32 verts (V, 3) and int64 faces (F, 3) on one CUDA device with the (name, tensor) pairs
+    `named`; the caller checks its own size limit."""
+    dev = _require_cuda(("verts", verts), ("faces", faces), *named)
+    _check_tensor("verts", verts, F32, (None, 3), "V, 3", op)
+    _check_tensor("faces", faces, I64, (None, 3), "F, 3", op)
+    return int(verts.shape[0]), int(faces.shape[0]), dev
+
+
+def _check_ranges(op, first_name, first, num_name, num):
+    """N of the int64 (N,) per-mesh ranges `first` and `num`."""
+    _check_tensor(first_name, first, I64, (None,), "N,", op)
+    N = int(first.shape[0])
+    _check_tensor(num_name, num, I64, (N,), "N,", op)
+    return N
+
+
+def _refuse_nondeterministic(op, why):
+    if torch.are_deterministic_algorithms_enabled() and not torch.is_deterministic_algorithms_warn_only_enabled():
+        raise RuntimeError("%s does not have a deterministic implementation (%s), but you set "
+                           "'torch.use_deterministic_algorithms(True)'." % (op, why))
+
+
+def _c(t):
+    return t.contiguous() if t is not None else None
+
+
 def _strides4(t):
-    import ctypes
     return (ctypes.c_int64 * 4)(*[int(v) for v in t.stride()])
 
 
-def _composite_forward(fn_name, features, alphas, points_idx):
-    dev = _require_cuda(("features", features), ("alphas", alphas), ("points_idx", points_idx))
-    if features.dtype != torch.float32 or alphas.dtype != torch.float32:
-        raise RuntimeError("expected scalar type Float")
-    if points_idx.dtype != torch.int64:
-        raise RuntimeError("expected scalar type Long but found %s" % points_idx.dtype)
-    if features.dim() != 2 or alphas.dim() != 4 or points_idx.dim() != 4 or alphas.shape != points_idx.shape:
-        raise RuntimeError("features must be (C, P); alphas and points_idx must both be (N, K, H, W)")
-    lib = _lib.load()
-    C, P = (int(v) for v in features.shape)
-    N, K, H, W = (int(v) for v in points_idx.shape)
-    feat = features.contiguous()
-    with torch.cuda.device(dev):
-        result = torch.empty((N, C, H, W), dtype=torch.float32, device=dev)
-        if result.numel() == 0:
-            return result
-        if K == 0:
-            return result.zero_()
-        _lib.check(getattr(lib, fn_name)(
-            _ptr(feat), C, P, alphas.data_ptr(), _strides4(alphas), points_idx.data_ptr(), _strides4(points_idx),
-            N, K, H, W, _ptr(result), _stream_ptr(dev)))
-    return result
-
-
-def _composite_backward(fn_name, grad_outputs, features, alphas, points_idx):
-    dev = _require_cuda(("grad_outputs", grad_outputs), ("features", features), ("alphas", alphas),
-                        ("points_idx", points_idx))
-    lib = _lib.load()
-    C, P = (int(v) for v in features.shape)
-    N, K, H, W = (int(v) for v in points_idx.shape)
-    feat, go = features.contiguous(), grad_outputs.contiguous()
-    with torch.cuda.device(dev):
-        grad_features = torch.empty((C, P), dtype=torch.float32, device=dev)
-        grad_alphas = torch.empty((N, K, H, W), dtype=torch.float32, device=dev)
-        if C * P == 0 or grad_alphas.numel() == 0:
-            return grad_features.zero_(), grad_alphas.zero_()
-        _lib.check(getattr(lib, fn_name)(
-            _ptr(go), _ptr(feat), C, P, alphas.data_ptr(), _strides4(alphas), points_idx.data_ptr(),
-            _strides4(points_idx), N, K, H, W, _ptr(grad_features), _ptr(grad_alphas), _stream_ptr(dev)))
-    return grad_features, grad_alphas
-
-
-def accum_alphacomposite(features: torch.Tensor, alphas: torch.Tensor, points_idx: torch.Tensor):
-    """pytorch3d._C.accum_alphacomposite (alphaCompositeForward, csrc/compositing/alpha_composite.h:59-82).
-
-    features (C,P) f32 (a (C,P) view of point-major memory -- what the renderer passes -- is read in place), alphas
-    (N,K,H,W) f32, points_idx (N,K,H,W) i64 (any strides) -> (N,C,H,W) f32."""
-    dev = _require_cuda(("features", features), ("alphas", alphas), ("points_idx", points_idx))
-    if features.dtype != torch.float32 or alphas.dtype != torch.float32:
-        raise RuntimeError("expected scalar type Float")
-    if points_idx.dtype != torch.int64:
-        raise RuntimeError("expected scalar type Long but found %s" % points_idx.dtype)
-    if features.dim() != 2 or alphas.dim() != 4 or points_idx.dim() != 4 or alphas.shape != points_idx.shape:
-        raise RuntimeError("features must be (C, P); alphas and points_idx must both be (N, K, H, W)")
-    lib = _lib.load()
-    C, P = (int(v) for v in features.shape)
-    N, K, H, W = (int(v) for v in points_idx.shape)
-    feat, fs_c, fs_p = _feature_layout(features)
-    with torch.cuda.device(dev):
-        result = torch.empty((N, C, H, W), dtype=torch.float32, device=dev)
-        if result.numel() == 0:
-            return result
-        if K == 0:
-            return result.zero_()
-        _lib.check(lib.b200r_alpha_composite_forward_strided(
-            _ptr(feat), C, P, fs_c, fs_p, alphas.data_ptr(), _strides4(alphas), points_idx.data_ptr(),
-            _strides4(points_idx), N, K, H, W, _ptr(result), _stream_ptr(dev)))
-    return result
-
-
-def accum_alphacomposite_backward(grad_outputs: torch.Tensor, features: torch.Tensor, alphas: torch.Tensor,
-                                  points_idx: torch.Tensor):
-    """pytorch3d._C.accum_alphacomposite_backward (alpha_composite.h:84-116) -> (grad_features, grad_alphas);
-    grad_features (C,P) has the memory layout of `features`."""
-    dev = _require_cuda(("grad_outputs", grad_outputs), ("features", features), ("alphas", alphas),
-                        ("points_idx", points_idx))
-    lib = _lib.load()
-    C, P = (int(v) for v in features.shape)
-    N, K, H, W = (int(v) for v in points_idx.shape)
-    feat, fs_c, fs_p = _feature_layout(features)
-    go = grad_outputs.contiguous()
-    with torch.cuda.device(dev):
-        if fs_c == 1 and C > 1:
-            grad_features = torch.empty((P, C), dtype=torch.float32, device=dev).permute(1, 0)
-        else:
-            grad_features = torch.empty((C, P), dtype=torch.float32, device=dev)
-        grad_alphas = torch.empty((N, K, H, W), dtype=torch.float32, device=dev)
-        if C * P == 0 or grad_alphas.numel() == 0:
-            return grad_features.zero_(), grad_alphas.zero_()
-        _lib.check(lib.b200r_alpha_composite_backward_strided(
-            _ptr(go), _ptr(feat), C, P, fs_c, fs_p, alphas.data_ptr(), _strides4(alphas), points_idx.data_ptr(),
-            _strides4(points_idx), N, K, H, W, grad_features.data_ptr(), _ptr(grad_alphas), _stream_ptr(dev)))
-    return grad_features, grad_alphas
+def _check_composite_inputs(features, weights, index, index_dtype, dims, grad=None):
+    """(C, P, device) of features (C, P) f32 and of the float32 per-slot weights (name, tensor) and `index_dtype`
+    per-slot indices (name, tensor), both of the 4-d shape `dims`; the upstream gradient (name, tensor), when given, is
+    only checked for its device here."""
+    dev = _require_cuda(*([grad] if grad is not None else []), ("features", features), weights, index)
+    _check_tensor("features", features, F32, (None, None), "C, P")
+    _check_tensor(*index, index_dtype, (None,) * 4, dims)
+    _check_tensor(*weights, F32, tuple(index[1].shape), dims)
+    return int(features.shape[0]), int(features.shape[1]), dev
 
 
 def _feature_layout(features):
@@ -286,28 +290,73 @@ def _feature_layout(features):
     return f, P, 1
 
 
+def _grad_features(layout, C, P, dev):
+    """grad_features (C, P) with the memory layout `features` was read in: point-major when it was read in place."""
+    if layout and layout[0] == 1 and C > 1:
+        return torch.empty((P, C), dtype=F32, device=dev).permute(1, 0)
+    return torch.empty((C, P), dtype=F32, device=dev)
+
+
+def _composite(name, features, alphas, points_idx, strided):
+    """The compositing forwards: alphas (N,K,H,W) f32, points_idx (N,K,H,W) i64 (any strides) -> (N,C,H,W) f32.  With
+    `strided` b200r_<name> takes the features' strides (see _feature_layout), else a contiguous (C, P) array."""
+    C, P, dev = _check_composite_inputs(features, ("alphas", alphas), ("points_idx", points_idx), I64, "N, K, H, W")
+    N, K, H, W = (int(v) for v in points_idx.shape)
+    feat, *layout = _feature_layout(features) if strided else (features.contiguous(),)
+    result = torch.empty((N, C, H, W), dtype=F32, device=dev)
+    if result.numel() == 0:
+        return result
+    if K == 0:
+        return result.zero_()
+    _launch(dev, name, _ptr(feat), C, P, *layout, alphas.data_ptr(), _strides4(alphas), points_idx.data_ptr(),
+            _strides4(points_idx), N, K, H, W, _ptr(result))
+    return result
+
+
+def _composite_grad(name, grad_outputs, features, alphas, points_idx, strided):
+    """The compositing backwards -> (grad_features (C,P) with the memory layout `features` is read in, grad_alphas)."""
+    C, P, dev = _check_composite_inputs(features, ("alphas", alphas), ("points_idx", points_idx), I64, "N, K, H, W",
+                                        ("grad_outputs", grad_outputs))
+    N, K, H, W = (int(v) for v in points_idx.shape)
+    _check_tensor("grad_outputs", grad_outputs, F32, (N, C, H, W), "N, C, H, W")
+    feat, *layout = _feature_layout(features) if strided else (features.contiguous(),)
+    go = grad_outputs.contiguous()
+    grad_features = _grad_features(layout, C, P, dev)
+    grad_alphas = torch.empty((N, K, H, W), dtype=F32, device=dev)
+    if C * P == 0 or grad_alphas.numel() == 0:
+        return grad_features.zero_(), grad_alphas.zero_()
+    _launch(dev, name, _ptr(go), _ptr(feat), C, P, *layout, alphas.data_ptr(), _strides4(alphas), points_idx.data_ptr(),
+            _strides4(points_idx), N, K, H, W, grad_features.data_ptr(), _ptr(grad_alphas))
+    return grad_features, grad_alphas
+
+
+def accum_alphacomposite(features: torch.Tensor, alphas: torch.Tensor, points_idx: torch.Tensor):
+    """pytorch3d._C.accum_alphacomposite (alphaCompositeForward, csrc/compositing/alpha_composite.h:59-82).
+
+    features (C,P) f32 (a (C,P) view of point-major memory -- what the renderer passes -- is read in place), alphas
+    (N,K,H,W) f32, points_idx (N,K,H,W) i64 (any strides) -> (N,C,H,W) f32."""
+    return _composite("alpha_composite_forward_strided", features, alphas, points_idx, True)
+
+
+def accum_alphacomposite_backward(grad_outputs: torch.Tensor, features: torch.Tensor, alphas: torch.Tensor,
+                                  points_idx: torch.Tensor):
+    """pytorch3d._C.accum_alphacomposite_backward (alpha_composite.h:84-116) -> (grad_features, grad_alphas);
+    grad_features (C,P) has the memory layout of `features`."""
+    return _composite_grad("alpha_composite_backward_strided", grad_outputs, features, alphas, points_idx, True)
+
+
 def points_alpha_render(features: torch.Tensor, idx: torch.Tensor, dists: torch.Tensor, radius: float):
     """Fused `accum_alphacomposite(features, 1 - dists / radius**2, idx)` on the rasterizer's own layout (no counterpart
     in pytorch3d._C; SURVEY.md 8f-2): features (C,P) f32, idx (N,H,W,K) i32, dists (N,H,W,K) f32 -> (N,C,H,W) f32."""
-    dev = _require_cuda(("features", features), ("idx", idx), ("dists", dists))
-    if features.dtype != torch.float32 or dists.dtype != torch.float32:
-        raise RuntimeError("expected scalar type Float")
-    if idx.dtype != torch.int32:
-        raise RuntimeError("expected scalar type Int but found %s" % idx.dtype)
-    if features.dim() != 2 or idx.dim() != 4 or idx.shape != dists.shape:
-        raise RuntimeError("features must be (C, P); idx and dists must both be (N, H, W, K)")
-    lib = _lib.load()
-    C, P = (int(v) for v in features.shape)
+    C, P, dev = _check_composite_inputs(features, ("dists", dists), ("idx", idx), I32, "N, H, W, K")
     N, H, W, K = (int(v) for v in idx.shape)
     feat, fs_c, fs_p = _feature_layout(features)
     ii, dd = idx.contiguous(), dists.contiguous()
-    with torch.cuda.device(dev):
-        images = torch.empty((N, C, H, W), dtype=torch.float32, device=dev)
-        if images.numel() == 0:
-            return images
-        _lib.check(lib.b200r_points_alpha_render_forward(_ptr(feat), C, P, fs_c, fs_p, _ptr(ii), _ptr(dd),
-                                                         float(radius) * float(radius), N, K, H, W, _ptr(images),
-                                                         _stream_ptr(dev)))
+    images = torch.empty((N, C, H, W), dtype=F32, device=dev)
+    if images.numel() == 0:
+        return images
+    _launch(dev, "points_alpha_render_forward", _ptr(feat), C, P, fs_c, fs_p, _ptr(ii), _ptr(dd),
+            float(radius) * float(radius), N, K, H, W, _ptr(images))
     return images
 
 
@@ -315,151 +364,141 @@ def points_alpha_render_backward(grad_images: torch.Tensor, features: torch.Tens
                                  dists: torch.Tensor, radius: float):
     """Backward of `points_alpha_render` -> (grad_features (C,P) with the memory layout of `features`, grad_dists
     (N,H,W,K))."""
-    dev = _require_cuda(("grad_images", grad_images), ("features", features), ("idx", idx), ("dists", dists))
-    lib = _lib.load()
-    C, P = (int(v) for v in features.shape)
+    C, P, dev = _check_composite_inputs(features, ("dists", dists), ("idx", idx), I32, "N, H, W, K",
+                                        ("grad_images", grad_images))
     N, H, W, K = (int(v) for v in idx.shape)
-    feat, fs_c, fs_p = _feature_layout(features)
+    _check_tensor("grad_images", grad_images, F32, (N, C, H, W), "N, C, H, W")
+    feat, *layout = _feature_layout(features)
     go, ii, dd = grad_images.contiguous(), idx.contiguous(), dists.contiguous()
-    with torch.cuda.device(dev):
-        if fs_c == 1 and C > 1:
-            grad_features = torch.empty((P, C), dtype=torch.float32, device=dev).permute(1, 0)  # point-major, like feat
-        else:
-            grad_features = torch.empty((C, P), dtype=torch.float32, device=dev)
-        grad_dists = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
-        if C * P == 0 or grad_dists.numel() == 0:
-            return grad_features.zero_(), grad_dists.zero_()
-        _lib.check(lib.b200r_points_alpha_render_backward(_ptr(go), _ptr(feat), C, P, fs_c, fs_p, _ptr(ii), _ptr(dd),
-                                                          float(radius) * float(radius), N, K, H, W,
-                                                          grad_features.data_ptr(), _ptr(grad_dists), _stream_ptr(dev)))
+    grad_features = _grad_features(layout, C, P, dev)
+    grad_dists = torch.empty((N, H, W, K), dtype=F32, device=dev)
+    if C * P == 0 or grad_dists.numel() == 0:
+        return grad_features.zero_(), grad_dists.zero_()
+    _launch(dev, "points_alpha_render_backward", _ptr(go), _ptr(feat), C, P, *layout, _ptr(ii), _ptr(dd),
+            float(radius) * float(radius), N, K, H, W, grad_features.data_ptr(), _ptr(grad_dists))
     return grad_features, grad_dists
 
 
 def accum_weightedsum(features: torch.Tensor, alphas: torch.Tensor, points_idx: torch.Tensor):
     """pytorch3d._C.accum_weightedsum (weightedSumForward, csrc/compositing/weighted_sum.h:57-78)."""
-    return _composite_forward("b200r_weighted_sum_forward", features, alphas, points_idx)
+    return _composite("weighted_sum_forward", features, alphas, points_idx, False)
 
 
 def accum_weightedsum_backward(grad_outputs: torch.Tensor, features: torch.Tensor, alphas: torch.Tensor,
                                points_idx: torch.Tensor):
     """pytorch3d._C.accum_weightedsum_backward (weighted_sum.h:80-110) -> (grad_features, grad_alphas)."""
-    return _composite_backward("b200r_weighted_sum_backward", grad_outputs, features, alphas, points_idx)
+    return _composite_grad("weighted_sum_backward", grad_outputs, features, alphas, points_idx, False)
 
 
 def accum_weightedsumnorm(features: torch.Tensor, alphas: torch.Tensor, points_idx: torch.Tensor):
     """pytorch3d._C.accum_weightedsumnorm (weightedSumNormForward, csrc/compositing/norm_weighted_sum.h:57-79)."""
-    return _composite_forward("b200r_norm_weighted_sum_forward", features, alphas, points_idx)
+    return _composite("norm_weighted_sum_forward", features, alphas, points_idx, False)
 
 
 def accum_weightedsumnorm_backward(grad_outputs: torch.Tensor, features: torch.Tensor, alphas: torch.Tensor,
                                    points_idx: torch.Tensor):
     """pytorch3d._C.accum_weightedsumnorm_backward (norm_weighted_sum.h:81-112) -> (grad_features, grad_alphas)."""
-    return _composite_backward("b200r_norm_weighted_sum_backward", grad_outputs, features, alphas, points_idx)
+    return _composite_grad("norm_weighted_sum_backward", grad_outputs, features, alphas, points_idx, False)
+
+
+def _check_interp_inputs(pix_to_face, barycentric_coords, face_attrs, grad_pix_attrs=None):
+    """(P, F, D, device), with the reference's shape errors (interp_face_attrs.cu)."""
+    dev = _require_cuda(("pix_to_face", pix_to_face), ("barycentric_coords", barycentric_coords),
+                        ("face_attributes", face_attrs),
+                        *([("pix_attrs", grad_pix_attrs)] if grad_pix_attrs is not None else []))
+    _check_tensor("pix_to_face", pix_to_face, I64, (None,), "P,")
+    _check_tensor("barycentric_coords", barycentric_coords, F32)
+    _check_tensor("face_attrs", face_attrs, F32)
+    P = int(pix_to_face.shape[0])
+    if tuple(barycentric_coords.shape) != (P, 3):
+        raise RuntimeError("barycentric_coords must have size (P, 3)")
+    if face_attrs.dim() != 3 or face_attrs.shape[1] != 3:
+        raise RuntimeError("face_attrs must have size (F, 3, D)")
+    F, D = int(face_attrs.shape[0]), int(face_attrs.shape[2])
+    if grad_pix_attrs is not None:
+        _check_tensor("grad_pix_attrs", grad_pix_attrs, F32)
+        if tuple(grad_pix_attrs.shape) != (P, D):
+            raise RuntimeError("grad_pix_attrs must have size (P, D)")
+    return P, F, D, dev
 
 
 def interp_face_attrs_forward(pix_to_face: torch.Tensor, barycentric_coords: torch.Tensor, face_attrs: torch.Tensor):
     """pytorch3d._C.interp_face_attrs_forward (csrc/interp_face_attrs/interp_face_attrs.h:45-66):
     pix_to_face (P,) i64, barycentric_coords (P,3) f32, face_attrs (F,3,D) f32 -> (P,D) f32."""
-    dev = _require_cuda(("pix_to_face", pix_to_face), ("barycentric_coords", barycentric_coords),
-                        ("face_attributes", face_attrs))
-    if barycentric_coords.dtype != torch.float32 or face_attrs.dtype != torch.float32:
-        raise RuntimeError("expected scalar type Float")
-    if pix_to_face.dtype != torch.int64:
-        raise RuntimeError("expected scalar type Long but found %s" % pix_to_face.dtype)
-    lib = _lib.load()
-    P, (F, _, D) = int(pix_to_face.shape[0]), (int(v) for v in face_attrs.shape)
+    P, F, D, dev = _check_interp_inputs(pix_to_face, barycentric_coords, face_attrs)
     p2f, bary, attrs = pix_to_face.contiguous(), barycentric_coords.contiguous(), face_attrs.contiguous()
-    with torch.cuda.device(dev):
-        out = torch.empty((P, D), dtype=torch.float32, device=dev)
-        if out.numel() == 0:
-            return out
-        _lib.check(lib.b200r_interp_face_attrs_forward(_ptr(p2f), _ptr(bary), _ptr(attrs), P, F, D, _ptr(out),
-                                                       _stream_ptr(dev)))
+    out = torch.empty((P, D), dtype=F32, device=dev)
+    if out.numel() == 0:
+        return out
+    _launch(dev, "interp_face_attrs_forward", _ptr(p2f), _ptr(bary), _ptr(attrs), P, F, D, _ptr(out))
     return out
 
 
 def interp_face_attrs_backward(pix_to_face: torch.Tensor, barycentric_coords: torch.Tensor, face_attrs: torch.Tensor,
                                grad_pix_attrs: torch.Tensor):
     """pytorch3d._C.interp_face_attrs_backward (interp_face_attrs.h:88-118) -> (grad_bary (P,3), grad_attrs (F,3,D))."""
-    dev = _require_cuda(("pix_to_face", pix_to_face), ("barycentric_coords", barycentric_coords),
-                        ("face_attributes", face_attrs), ("pix_attrs", grad_pix_attrs))
-    lib = _lib.load()
-    P, (F, _, D) = int(pix_to_face.shape[0]), (int(v) for v in face_attrs.shape)
+    P, F, D, dev = _check_interp_inputs(pix_to_face, barycentric_coords, face_attrs, grad_pix_attrs)
     p2f, bary, attrs = pix_to_face.contiguous(), barycentric_coords.contiguous(), face_attrs.contiguous()
     gp = grad_pix_attrs.contiguous()
-    with torch.cuda.device(dev):
-        grad_bary = torch.empty((P, 3), dtype=torch.float32, device=dev)
-        grad_attrs = torch.empty((F, 3, D), dtype=torch.float32, device=dev)
-        if grad_attrs.numel() == 0 or P == 0:
-            return grad_bary.zero_(), grad_attrs.zero_()
-        _lib.check(lib.b200r_interp_face_attrs_backward(_ptr(p2f), _ptr(bary), _ptr(attrs), _ptr(gp), P, F, D,
-                                                        _ptr(grad_bary), _ptr(grad_attrs), _stream_ptr(dev)))
+    grad_bary = torch.empty((P, 3), dtype=F32, device=dev)
+    grad_attrs = torch.empty((F, 3, D), dtype=F32, device=dev)
+    if grad_attrs.numel() == 0 or P == 0:
+        return grad_bary.zero_(), grad_attrs.zero_()
+    _launch(dev, "interp_face_attrs_backward", _ptr(p2f), _ptr(bary), _ptr(attrs), _ptr(gp), P, F, D, _ptr(grad_bary),
+            _ptr(grad_attrs))
     return grad_bary, grad_attrs
 
 
-_SCALAR_TYPE_NAMES = {torch.int64: "Long", torch.bool: "Bool"}
-
-
-def _check_blend_inputs(named_floats, pix_to_face, index_name="pix_to_face", index_dtype=torch.int64):
-    """float32 CUDA tensors on one device, and an (N, H, W, K) per-slot tensor `index_name` of `index_dtype` (the face
-    indices, or the splatter blend's background mask)."""
-    dev = _require_cuda(*named_floats, (index_name, pix_to_face))
-    for name, t in named_floats:
-        if t.dtype != torch.float32:
-            raise RuntimeError("Expected tensor for %s to have scalar type Float; but got %s" % (name, t.dtype))
-    if pix_to_face.dtype != index_dtype:
-        raise RuntimeError("expected scalar type %s but found %s" % (_SCALAR_TYPE_NAMES[index_dtype], pix_to_face.dtype))
+def _check_index(pix_to_face, name="pix_to_face", dtype=I64):
+    """The (N, H, W, K) of the per-slot tensor `name` of `dtype` (the face indices, or the splatter blend's background
+    mask); dtype None checks the shape alone."""
+    _check_tensor(name, pix_to_face, dtype)
     if pix_to_face.dim() != 4:
-        raise RuntimeError("%s must have dimensions (N, H, W, K)" % index_name)
-    return dev
+        raise RuntimeError("%s must have dimensions (N, H, W, K), got %s" % (name, tuple(pix_to_face.shape)))
+    return tuple(pix_to_face.shape)
 
 
 def sigmoid_alpha_blend(dists: torch.Tensor, pix_to_face: torch.Tensor, sigma: float):
     """pytorch3d._C.sigmoid_alpha_blend (SigmoidAlphaBlend, csrc/blending/sigmoid_alpha_blend.h): dists (N,H,W,K) f32,
     pix_to_face (N,H,W,K) i64 -> alphas (N,H,W) f32, bit-identical to the reference's CUDA kernel."""
-    dev = _check_blend_inputs([("distances", dists)], pix_to_face)
-    if dists.shape != pix_to_face.shape:
-        raise RuntimeError("distances and pix_to_face must both be (N, H, W, K)")
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    dev = _require_cuda(("distances", dists), ("pix_to_face", pix_to_face))
+    N, H, W, K = _check_index(pix_to_face)
+    _check_float("distances", dists, (N, H, W, K), "N, H, W, K")
     dd, p2f = dists.contiguous(), pix_to_face.contiguous()
-    with torch.cuda.device(dev):
-        alphas = torch.empty((N, H, W), dtype=torch.float32, device=dev)
-        if alphas.numel() == 0:
-            return alphas
-        _lib.check(lib.b200r_sigmoid_alpha_blend_forward(_ptr(dd), _ptr(p2f), N, H, W, K, float(sigma), _ptr(alphas),
-                                                         _stream_ptr(dev)))
+    alphas = torch.empty((N, H, W), dtype=F32, device=dev)
+    if alphas.numel() == 0:
+        return alphas
+    _launch(dev, "sigmoid_alpha_blend_forward", _ptr(dd), _ptr(p2f), N, H, W, K, float(sigma), _ptr(alphas))
     return alphas
 
 
 def sigmoid_alpha_blend_backward(grad_alphas: torch.Tensor, alphas: torch.Tensor, dists: torch.Tensor,
                                  pix_to_face: torch.Tensor, sigma: float):
     """pytorch3d._C.sigmoid_alpha_blend_backward (SigmoidAlphaBlendBackward) -> grad_dists (N,H,W,K) f32."""
-    dev = _check_blend_inputs([("grad_alphas", grad_alphas), ("alphas", alphas), ("distances", dists)], pix_to_face)
-    if dists.shape != pix_to_face.shape or alphas.shape != pix_to_face.shape[:3] or grad_alphas.shape != alphas.shape:
-        raise RuntimeError("distances and pix_to_face must be (N, H, W, K); alphas and grad_alphas (N, H, W)")
+    dev = _require_cuda(("grad_alphas", grad_alphas), ("alphas", alphas), ("distances", dists),
+                        ("pix_to_face", pix_to_face))
+    N, H, W, K = _check_index(pix_to_face)
+    _check_float("distances", dists, (N, H, W, K), "N, H, W, K")
+    _check_float("alphas", alphas, (N, H, W), "N, H, W")
+    _check_float("grad_alphas", grad_alphas, (N, H, W), "N, H, W")
     if alphas.numel() == 0:
         return grad_alphas  # what the reference returns for an empty image (sigmoid_alpha_blend.cu)
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
     ga, al, dd, p2f = grad_alphas.contiguous(), alphas.contiguous(), dists.contiguous(), pix_to_face.contiguous()
-    with torch.cuda.device(dev):
-        grad_dists = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
-        if grad_dists.numel() == 0:
-            return grad_dists
-        _lib.check(lib.b200r_sigmoid_alpha_blend_backward(_ptr(ga), _ptr(al), _ptr(dd), _ptr(p2f), N, H, W, K,
-                                                          float(sigma), _ptr(grad_dists), _stream_ptr(dev)))
+    grad_dists = torch.empty((N, H, W, K), dtype=F32, device=dev)
+    if grad_dists.numel() == 0:
+        return grad_dists
+    _launch(dev, "sigmoid_alpha_blend_backward", _ptr(ga), _ptr(al), _ptr(dd), _ptr(p2f), N, H, W, K, float(sigma),
+            _ptr(grad_dists))
     return grad_dists
 
 
 def _softmax_side_args(dev, N, background_color, znear, zfar):
     """(background ptr, host background value, znear ptr, zfar ptr, znear value, zfar value, tensors to keep alive).
     Tensors are read on the device; Python numbers go to the kernel as numbers."""
-    import ctypes
     keep = []
     if torch.is_tensor(background_color):
         bg = background_color
-        if bg.device != dev or bg.dtype != torch.float32 or bg.numel() != 3:
+        if bg.device != dev or bg.dtype != F32 or bg.numel() != 3:
             raise RuntimeError("background_color must be a float32 tensor of 3 values on %s" % dev)
         bg = bg.reshape(3).contiguous()
         keep.append(bg)
@@ -472,7 +511,7 @@ def _softmax_side_args(dev, N, background_color, znear, zfar):
     ptrs, values = [], []
     for name, z in (("znear", znear), ("zfar", zfar)):
         if torch.is_tensor(z):
-            if z.device != dev or z.dtype != torch.float32 or z.dim() != 1 or z.shape[0] not in (1, N):
+            if z.device != dev or z.dtype != F32 or z.dim() != 1 or z.shape[0] not in (1, N):
                 raise RuntimeError("%s must be a number or a float32 tensor of shape (N,) on %s" % (name, dev))
             z = z.expand(N).contiguous()
             keep.append(z)
@@ -484,14 +523,18 @@ def _softmax_side_args(dev, N, background_color, znear, zfar):
     return bg_ptr, bg_val, ptrs[0], ptrs[1], values[0], values[1], keep
 
 
-def _check_softmax_inputs(colors, pix_to_face, zbuf, dists):
-    dev = _check_blend_inputs([("colors", colors), ("zbuf", zbuf), ("dists", dists)], pix_to_face)
-    shape = pix_to_face.shape
-    if zbuf.shape != shape or dists.shape != shape or colors.shape != shape + (3,):
-        raise RuntimeError("pix_to_face, zbuf and dists must be (N, H, W, K) and colors (N, H, W, K, 3)")
+def _check_softmax_inputs(colors, pix_to_face, zbuf, dists, grad_out=None):
+    dev = _require_cuda(*([("grad_out", grad_out)] if grad_out is not None else []), ("colors", colors),
+                        ("zbuf", zbuf), ("dists", dists), ("pix_to_face", pix_to_face))
+    shape = _check_index(pix_to_face)
+    _check_float("colors", colors, shape + (3,), "N, H, W, K, 3")
+    _check_float("zbuf", zbuf, shape, "N, H, W, K")
+    _check_float("dists", dists, shape, "N, H, W, K")
+    if grad_out is not None:
+        _check_float("grad_out", grad_out, shape[:3] + (4,), "N, H, W, 4")
     if shape[3] > kMaxPointsPerPixel:
         raise RuntimeError("Must have faces_per_pixel <= %d" % kMaxPointsPerPixel)
-    return dev
+    return shape + (dev,)
 
 
 def softmax_rgb_blend(colors: torch.Tensor, pix_to_face: torch.Tensor, zbuf: torch.Tensor, dists: torch.Tensor,
@@ -499,18 +542,14 @@ def softmax_rgb_blend(colors: torch.Tensor, pix_to_face: torch.Tensor, zbuf: tor
     """Fused pytorch3d.renderer.blending.softmax_rgb_blend on the rasterizer's layout (no counterpart in pytorch3d._C;
     SURVEY.md 8f-5): colors (N,H,W,K,3) f32, pix_to_face (N,H,W,K) i64, zbuf / dists (N,H,W,K) f32; background_color a
     float32 CUDA tensor of 3 values or 3 numbers; znear / zfar numbers or float32 (N,) CUDA tensors -> (N,H,W,4) f32."""
-    dev = _check_softmax_inputs(colors, pix_to_face, zbuf, dists)
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    N, H, W, K, dev = _check_softmax_inputs(colors, pix_to_face, zbuf, dists)
     bg_ptr, bg_val, zn_ptr, zf_ptr, zn, zf, keep = _softmax_side_args(dev, N, background_color, znear, zfar)
     c, p2f, zb, dd = colors.contiguous(), pix_to_face.contiguous(), zbuf.contiguous(), dists.contiguous()
-    with torch.cuda.device(dev):
-        out = torch.empty((N, H, W, 4), dtype=torch.float32, device=dev)
-        if out.numel() == 0:
-            return out
-        _lib.check(lib.b200r_softmax_rgb_blend_forward(
-            _ptr(c), _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K, float(sigma), float(gamma), bg_ptr, bg_val, zn_ptr,
-            zf_ptr, zn, zf, _ptr(out), _stream_ptr(dev)))
+    out = torch.empty((N, H, W, 4), dtype=F32, device=dev)
+    if out.numel() == 0:
+        return out
+    _launch(dev, "softmax_rgb_blend_forward", _ptr(c), _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K, float(sigma),
+            float(gamma), bg_ptr, bg_val, zn_ptr, zf_ptr, zn, zf, _ptr(out))
     del keep
     return out
 
@@ -519,24 +558,18 @@ def softmax_rgb_blend_backward(grad_out: torch.Tensor, colors: torch.Tensor, pix
                                zbuf: torch.Tensor, dists: torch.Tensor, sigma: float, gamma: float, background_color,
                                znear=1.0, zfar=100.0):
     """Backward of `softmax_rgb_blend` -> (grad_colors (N,H,W,K,3), grad_dists (N,H,W,K), grad_zbuf (N,H,W,K))."""
-    dev = _check_softmax_inputs(colors, pix_to_face, zbuf, dists)
-    _require_cuda(("grad_out", grad_out), ("colors", colors))
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
-    if grad_out.dtype != torch.float32 or tuple(grad_out.shape) != (N, H, W, 4):
-        raise RuntimeError("grad_out must be a float32 tensor of shape (N, H, W, 4)")
-    lib = _lib.load()
+    N, H, W, K, dev = _check_softmax_inputs(colors, pix_to_face, zbuf, dists, grad_out)
     bg_ptr, bg_val, zn_ptr, zf_ptr, zn, zf, keep = _softmax_side_args(dev, N, background_color, znear, zfar)
     go = grad_out.contiguous()
     c, p2f, zb, dd = colors.contiguous(), pix_to_face.contiguous(), zbuf.contiguous(), dists.contiguous()
-    with torch.cuda.device(dev):
-        grad_colors = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev)
-        grad_dists = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
-        grad_zbuf = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
-        if grad_dists.numel() == 0:
-            return grad_colors, grad_dists, grad_zbuf
-        _lib.check(lib.b200r_softmax_rgb_blend_backward(
-            _ptr(go), _ptr(c), _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K, float(sigma), float(gamma), bg_ptr, bg_val,
-            zn_ptr, zf_ptr, zn, zf, _ptr(grad_colors), _ptr(grad_dists), _ptr(grad_zbuf), _stream_ptr(dev)))
+    grad_colors = torch.empty((N, H, W, K, 3), dtype=F32, device=dev)
+    grad_dists = torch.empty((N, H, W, K), dtype=F32, device=dev)
+    grad_zbuf = torch.empty((N, H, W, K), dtype=F32, device=dev)
+    if grad_dists.numel() == 0:
+        return grad_colors, grad_dists, grad_zbuf
+    _launch(dev, "softmax_rgb_blend_backward", _ptr(go), _ptr(c), _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K,
+            float(sigma), float(gamma), bg_ptr, bg_val, zn_ptr, zf_ptr, zn, zf, _ptr(grad_colors), _ptr(grad_dists),
+            _ptr(grad_zbuf))
     del keep
     return grad_colors, grad_dists, grad_zbuf
 
@@ -545,44 +578,40 @@ def _depth_zfar_arg(dev, zfar):
     """(zfar ptr, zfar value, tensor to keep alive).  A 1-element float32 tensor on `dev` is read on the device; a
     Python number goes to the kernel as a number."""
     if torch.is_tensor(zfar):
-        if zfar.device != dev or zfar.dtype != torch.float32 or zfar.numel() != 1:
+        if zfar.device != dev or zfar.dtype != F32 or zfar.numel() != 1:
             raise RuntimeError("zfar must be a number or a 1-element float32 tensor on %s" % dev)
         z = zfar.reshape(1).contiguous()
         return z.data_ptr(), 0.0, z
     return None, float(zfar), None
 
 
-def _check_depth_inputs(pix_to_face, named_floats):
-    dev = _check_blend_inputs(named_floats, pix_to_face)
+def _check_depth_inputs(pix_to_face, named_floats, grad_out=None):
+    """(N, H, W, K, device) of pix_to_face and the float32 (N, H, W, K) tensors `named_floats`, and of the float32
+    (N, H, W, 1) grad_out when given."""
+    dev = _require_cuda(*([("grad_out", grad_out)] if grad_out is not None else []), *named_floats,
+                        ("pix_to_face", pix_to_face))
+    shape = _check_index(pix_to_face)
     for name, t in named_floats:
-        if t.shape != pix_to_face.shape:
-            raise RuntimeError("pix_to_face and %s must both be (N, H, W, K)" % name)
-    if not 1 <= pix_to_face.shape[3] <= kMaxPointsPerPixel:
+        _check_float(name, t, shape, "N, H, W, K")
+    if grad_out is not None:
+        _check_float("grad_out", grad_out, shape[:3] + (1,), "N, H, W, 1")
+    if not 1 <= shape[3] <= kMaxPointsPerPixel:
         raise RuntimeError("Must have 1 <= faces_per_pixel <= %d" % kMaxPointsPerPixel)
-    return dev
-
-
-def _check_depth_grad(grad_out, pix_to_face):
-    _require_cuda(("grad_out", grad_out), ("pix_to_face", pix_to_face))
-    if grad_out.dtype != torch.float32 or tuple(grad_out.shape) != tuple(pix_to_face.shape[:3]) + (1,):
-        raise RuntimeError("grad_out must be a float32 tensor of shape (N, H, W, 1)")
+    return shape + (dev,)
 
 
 def soft_depth_blend(pix_to_face: torch.Tensor, zbuf: torch.Tensor, dists: torch.Tensor, sigma: float, zfar):
     """Fused SoftDepthShader of pytorch3d/renderer/mesh/shader.py on the rasterizer's layout (no counterpart in
     pytorch3d._C): pix_to_face (N,H,W,K) i64, zbuf / dists (N,H,W,K) f32, 1 <= K <= 150; zfar a number or a 1-element
     float32 tensor on the same device -> (N,H,W,1) f32."""
-    dev = _check_depth_inputs(pix_to_face, [("zbuf", zbuf), ("dists", dists)])
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    N, H, W, K, dev = _check_depth_inputs(pix_to_face, [("zbuf", zbuf), ("dists", dists)])
     zf_ptr, zf, keep = _depth_zfar_arg(dev, zfar)
     p2f, zb, dd = pix_to_face.contiguous(), zbuf.contiguous(), dists.contiguous()
-    with torch.cuda.device(dev):
-        out = torch.empty((N, H, W, 1), dtype=torch.float32, device=dev)
-        if out.numel() == 0:
-            return out
-        _lib.check(lib.b200r_soft_depth_blend_forward(_ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K, float(sigma), zf_ptr,
-                                                      zf, _ptr(out), _stream_ptr(dev)))
+    out = torch.empty((N, H, W, 1), dtype=F32, device=dev)
+    if out.numel() == 0:
+        return out
+    _launch(dev, "soft_depth_blend_forward", _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K, float(sigma), zf_ptr, zf,
+            _ptr(out))
     del keep
     return out
 
@@ -590,20 +619,15 @@ def soft_depth_blend(pix_to_face: torch.Tensor, zbuf: torch.Tensor, dists: torch
 def soft_depth_blend_backward(grad_out: torch.Tensor, pix_to_face: torch.Tensor, zbuf: torch.Tensor,
                               dists: torch.Tensor, sigma: float, zfar):
     """Backward of `soft_depth_blend` -> (grad_zbuf (N,H,W,K), grad_dists (N,H,W,K))."""
-    dev = _check_depth_inputs(pix_to_face, [("zbuf", zbuf), ("dists", dists)])
-    _check_depth_grad(grad_out, pix_to_face)
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    N, H, W, K, dev = _check_depth_inputs(pix_to_face, [("zbuf", zbuf), ("dists", dists)], grad_out)
     zf_ptr, zf, keep = _depth_zfar_arg(dev, zfar)
     go, p2f, zb, dd = grad_out.contiguous(), pix_to_face.contiguous(), zbuf.contiguous(), dists.contiguous()
-    with torch.cuda.device(dev):
-        grad_zbuf = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
-        grad_dists = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
-        if grad_zbuf.numel() == 0:
-            return grad_zbuf, grad_dists
-        _lib.check(lib.b200r_soft_depth_blend_backward(_ptr(go), _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K,
-                                                       float(sigma), zf_ptr, zf, _ptr(grad_zbuf), _ptr(grad_dists),
-                                                       _stream_ptr(dev)))
+    grad_zbuf = torch.empty((N, H, W, K), dtype=F32, device=dev)
+    grad_dists = torch.empty((N, H, W, K), dtype=F32, device=dev)
+    if grad_zbuf.numel() == 0:
+        return grad_zbuf, grad_dists
+    _launch(dev, "soft_depth_blend_backward", _ptr(go), _ptr(p2f), _ptr(zb), _ptr(dd), N, H, W, K, float(sigma), zf_ptr,
+            zf, _ptr(grad_zbuf), _ptr(grad_dists))
     del keep
     return grad_zbuf, grad_dists
 
@@ -611,50 +635,43 @@ def soft_depth_blend_backward(grad_out: torch.Tensor, pix_to_face: torch.Tensor,
 def hard_depth(pix_to_face: torch.Tensor, zbuf: torch.Tensor, zfar):
     """Fused HardDepthShader of pytorch3d/renderer/mesh/shader.py: zbuf of slot 0 where pix_to_face of slot 0 is valid,
     zfar elsewhere.  pix_to_face (N,H,W,K) i64, zbuf (N,H,W,K) f32; zfar as for `soft_depth_blend` -> (N,H,W,1) f32."""
-    dev = _check_depth_inputs(pix_to_face, [("zbuf", zbuf)])
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    N, H, W, K, dev = _check_depth_inputs(pix_to_face, [("zbuf", zbuf)])
     zf_ptr, zf, keep = _depth_zfar_arg(dev, zfar)
     p2f, zb = pix_to_face.contiguous(), zbuf.contiguous()
-    with torch.cuda.device(dev):
-        out = torch.empty((N, H, W, 1), dtype=torch.float32, device=dev)
-        if out.numel() == 0:
-            return out
-        _lib.check(lib.b200r_hard_depth_forward(_ptr(p2f), _ptr(zb), N, H, W, K, zf_ptr, zf, _ptr(out),
-                                                _stream_ptr(dev)))
+    out = torch.empty((N, H, W, 1), dtype=F32, device=dev)
+    if out.numel() == 0:
+        return out
+    _launch(dev, "hard_depth_forward", _ptr(p2f), _ptr(zb), N, H, W, K, zf_ptr, zf, _ptr(out))
     del keep
     return out
 
 
 def hard_depth_backward(grad_out: torch.Tensor, pix_to_face: torch.Tensor):
     """Backward of `hard_depth` -> grad_zbuf (N,H,W,K): grad_out on slot 0 of valid pixels, 0 everywhere else."""
-    _check_depth_inputs(pix_to_face, [])
-    _check_depth_grad(grad_out, pix_to_face)
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
+    N, H, W, K, dev = _check_depth_inputs(pix_to_face, [], grad_out)
     go, p2f = grad_out.contiguous(), pix_to_face.contiguous()
-    dev = pix_to_face.device
-    with torch.cuda.device(dev):
-        grad_zbuf = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
-        if grad_zbuf.numel() == 0:
-            return grad_zbuf
-        _lib.check(lib.b200r_hard_depth_backward(_ptr(go), _ptr(p2f), N, H, W, K, _ptr(grad_zbuf), _stream_ptr(dev)))
+    grad_zbuf = torch.empty((N, H, W, K), dtype=F32, device=dev)
+    if grad_zbuf.numel() == 0:
+        return grad_zbuf
+    _launch(dev, "hard_depth_backward", _ptr(go), _ptr(p2f), N, H, W, K, _ptr(grad_zbuf))
     return grad_zbuf
 
 
-def _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma):
-    dev = _check_blend_inputs([("colors", colors), ("pixel_coords_screen", pixel_coords_screen)], background_mask,
-                              "background_mask", torch.bool)
-    shape = tuple(background_mask.shape)
-    if colors.shape != shape + (3,) or pixel_coords_screen.shape != shape + (3,):
-        raise RuntimeError("background_mask must be (N, H, W, K), colors and pixel_coords_screen (N, H, W, K, 3)")
+def _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma, grad_out=None):
+    dev = _require_cuda(*([("grad_out", grad_out)] if grad_out is not None else []), ("colors", colors),
+                        ("pixel_coords_screen", pixel_coords_screen), ("background_mask", background_mask))
+    shape = _check_index(background_mask, "background_mask", torch.bool)
+    _check_float("colors", colors, shape + (3,), "N, H, W, K, 3")
+    _check_float("pixel_coords_screen", pixel_coords_screen, shape + (3,), "N, H, W, K, 3")
+    if grad_out is not None:
+        _check_float("grad_out", grad_out, shape[:3] + (4,), "N, H, W, 4")
     if shape[3] > kMaxPointsPerPixel:
         raise RuntimeError("Must have faces_per_pixel <= %d" % kMaxPointsPerPixel)
     if shape[3] < 1:
         raise RuntimeError("faces_per_pixel must be at least 1")
     if not float(sigma) > 0.0:
         raise RuntimeError("Only positive standard deviations make sense.")
-    return dev
+    return shape + (dev,)
 
 
 def splatter_blend(colors: torch.Tensor, pixel_coords_screen: torch.Tensor, background_mask: torch.Tensor,
@@ -662,17 +679,14 @@ def splatter_blend(colors: torch.Tensor, pixel_coords_screen: torch.Tensor, back
     """Fused splatter blend (the blend of pytorch3d.renderer.splatter_blend.SplatterBlender after its projection step;
     no counterpart in pytorch3d._C): colors and pixel_coords_screen (N,H,W,K,3) f32, background_mask (N,H,W,K) bool,
     sigma > 0 in pixels; background_color a float32 CUDA tensor of 3 values or 3 numbers -> (N,H,W,4) f32 RGBA."""
-    dev = _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma)
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in background_mask.shape)
+    N, H, W, K, dev = _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma)
     bg_ptr, bg_val, _, _, _, _, keep = _softmax_side_args(dev, N, background_color, 1.0, 100.0)
     c, xyz, m = colors.contiguous(), pixel_coords_screen.contiguous(), background_mask.contiguous()
-    with torch.cuda.device(dev):
-        out = torch.empty((N, H, W, 4), dtype=torch.float32, device=dev)
-        if out.numel() == 0:
-            return out
-        _lib.check(lib.b200r_splatter_blend_forward(_ptr(c), _ptr(xyz), _ptr(m), N, H, W, K, float(sigma), bg_ptr,
-                                                    bg_val, _ptr(out), _stream_ptr(dev)))
+    out = torch.empty((N, H, W, 4), dtype=F32, device=dev)
+    if out.numel() == 0:
+        return out
+    _launch(dev, "splatter_blend_forward", _ptr(c), _ptr(xyz), _ptr(m), N, H, W, K, float(sigma), bg_ptr, bg_val,
+            _ptr(out))
     del keep
     return out
 
@@ -681,25 +695,17 @@ def splatter_blend_backward(grad_out: torch.Tensor, colors: torch.Tensor, pixel_
                             background_mask: torch.Tensor, sigma: float, background_color):
     """Backward of `splatter_blend` -> (grad_colors (N,H,W,K,3), grad_pixel_coords_screen (N,H,W,K,3)); both are 0 in
     background slots, and the z channel of grad_pixel_coords_screen is 0."""
-    dev = _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma)
-    _require_cuda(("grad_out", grad_out), ("colors", colors))
-    N, H, W, K = (int(v) for v in background_mask.shape)
-    if grad_out.dtype != torch.float32 or tuple(grad_out.shape) != (N, H, W, 4):
-        raise RuntimeError("grad_out must be a float32 tensor of shape (N, H, W, 4)")
-    lib = _lib.load()
+    N, H, W, K, dev = _check_splatter_inputs(colors, pixel_coords_screen, background_mask, sigma, grad_out)
     bg_ptr, bg_val, _, _, _, _, keep = _softmax_side_args(dev, N, background_color, 1.0, 100.0)
     go = grad_out.contiguous()
     c, xyz, m = colors.contiguous(), pixel_coords_screen.contiguous(), background_mask.contiguous()
-    with torch.cuda.device(dev):
-        grad_colors = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev)
-        grad_xyz = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev)
-        if grad_colors.numel() == 0:
-            return grad_colors, grad_xyz
-        ws_bytes = int(lib.b200r_splatter_blend_workspace_bytes(N, H, W))
-        workspace = torch.empty((ws_bytes // 4,), dtype=torch.float32, device=dev)  # caching allocator: 512-byte aligned
-        _lib.check(lib.b200r_splatter_blend_backward(
-            _ptr(go), _ptr(c), _ptr(xyz), _ptr(m), N, H, W, K, float(sigma), bg_ptr, bg_val, _ptr(workspace), ws_bytes,
-            _ptr(grad_colors), _ptr(grad_xyz), _stream_ptr(dev)))
+    grad_colors = torch.empty((N, H, W, K, 3), dtype=F32, device=dev)
+    grad_xyz = torch.empty((N, H, W, K, 3), dtype=F32, device=dev)
+    if grad_colors.numel() == 0:
+        return grad_colors, grad_xyz
+    ws, ws_bytes = _workspace(dev, "splatter_blend", N, H, W)
+    _launch(dev, "splatter_blend_backward", _ptr(go), _ptr(c), _ptr(xyz), _ptr(m), N, H, W, K, float(sigma), bg_ptr,
+            bg_val, _ptr(ws), ws_bytes, _ptr(grad_colors), _ptr(grad_xyz))
     del keep
     return grad_colors, grad_xyz
 
@@ -708,37 +714,37 @@ SHADING_PARAMS = 22  # B200R_SHADING_PARAMS: the per-image parameter row of the 
 LIGHT_KINDS = {"point": 0, "directional": 1, "ambient": 2}  # B200R_LIGHT_*
 
 
-def _check_shading_inputs(pix_to_face, barycentric_coords, face_positions, face_normals, texels, params, flat, light):
-    """The (N, H, W, K) shape; raises RuntimeError naming the argument for anything the kernels cannot take."""
+def _check_shading_inputs(pix_to_face, barycentric_coords, face_positions, face_normals, texels, params, flat, light,
+                          grads=()):
+    """(N, H, W, K, F, device); raises RuntimeError naming the argument for anything the kernels cannot take.  `grads`
+    are the (name, tensor) upstream gradients, float32 (N, H, W, K, 3) or None."""
     if light not in LIGHT_KINDS:
         raise RuntimeError("light must be one of %s, got %r" % (sorted(LIGHT_KINDS), light))
     if light != "ambient" and face_normals is None:
         raise RuntimeError("face_normals are required for %s light" % light)
     if not flat and barycentric_coords is None:
         raise RuntimeError("barycentric_coords are required for phong shading")
-    floats =[("texels", texels), ("params", params), ("face_positions", face_positions)]
+    grads = [(name, t) for name, t in grads if t is not None]
+    floats = [("texels", texels), ("params", params), ("face_positions", face_positions)]
     if not flat:
         floats.append(("barycentric_coords", barycentric_coords))
     if light != "ambient":
         floats.append(("face_normals", face_normals))
-    dev = _check_blend_inputs(floats, pix_to_face)
-    shape = tuple(pix_to_face.shape)
-    if tuple(texels.shape) != shape + (3,):
-        raise RuntimeError("texels must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
-                           % (tuple(texels.shape),))
-    if not flat and tuple(barycentric_coords.shape) != shape + (3,):
-        raise RuntimeError("barycentric_coords must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
-                           % (tuple(barycentric_coords.shape),))
+    dev = _require_cuda(*grads, *floats, ("pix_to_face", pix_to_face))
+    shape = _check_index(pix_to_face)
+    _check_float("texels", texels, shape + (3,), "N, H, W, K, 3")
+    if not flat:
+        _check_float("barycentric_coords", barycentric_coords, shape + (3,), "N, H, W, K, 3")
     face_shape = (3,) if flat else (3, 3)
-    for name, t in (("face_positions", face_positions), ("face_normals", face_normals)):
-        if t is not None and (t.dim() != 1 + len(face_shape) or tuple(t.shape[1:]) != face_shape):
-            raise RuntimeError("%s must be (F, %s), got %s"
-                               % (name, ", ".join(str(v) for v in face_shape), tuple(t.shape)))
-    if light != "ambient" and face_normals.shape[0] != face_positions.shape[0]:
-        raise RuntimeError("face_positions and face_normals must have the same number of faces")
-    if tuple(params.shape) != (shape[0], SHADING_PARAMS):
-        raise RuntimeError("params must be (N, %d), got %s" % (SHADING_PARAMS, tuple(params.shape)))
-    return dev
+    face_dims = "F, 3" if flat else "F, 3, 3"
+    _check_float("face_positions", face_positions, (None,) + face_shape, face_dims)
+    F = int(face_positions.shape[0])
+    if light != "ambient":
+        _check_float("face_normals", face_normals, (F,) + face_shape, face_dims)
+    _check_float("params", params, (shape[0], SHADING_PARAMS), "N, %d" % SHADING_PARAMS)
+    for name, t in grads:
+        _check_float(name, t, shape + (3,), "N, H, W, K, 3")
+    return shape + (F, dev)
 
 
 def shading_forward(pix_to_face: torch.Tensor, barycentric_coords, face_positions: torch.Tensor, face_normals,
@@ -748,23 +754,23 @@ def shading_forward(pix_to_face: torch.Tensor, barycentric_coords, face_position
     or (F,3) (flat), face_normals unused (may be None) for ambient light; texels (N,H,W,K,3) f32; params (N,22) f32 (the
     row of include/b200_raster.h); light "point", "directional" or "ambient".
     -> (colors (N,H,W,K,3), positions (N,H,W,K,3) or None)."""
-    dev = _check_shading_inputs(pix_to_face, barycentric_coords, face_positions, face_normals, texels, params, flat,
-                                light)
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
-    F = int(face_positions.shape[0])
+    N, H, W, K, F, dev = _check_shading_inputs(pix_to_face, barycentric_coords, face_positions, face_normals, texels,
+                                               params, flat, light)
     p2f, tx, prm, fp = pix_to_face.contiguous(), texels.contiguous(), params.contiguous(), face_positions.contiguous()
     bary = None if flat else barycentric_coords.contiguous()
     fn = None if light == "ambient" else face_normals.contiguous()
-    with torch.cuda.device(dev):
-        colors = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev)
-        positions = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev) if return_positions else None
-        if colors.numel() == 0:
-            return colors, positions
-        _lib.check(lib.b200r_shading_forward(_ptr(p2f), _ptr(bary), _ptr(fp), _ptr(fn), F, _ptr(tx), _ptr(prm), N, H,
-                                             W, K, int(bool(flat)), LIGHT_KINDS[light], _ptr(colors), _ptr(positions),
-                                             _stream_ptr(dev)))
+    colors = torch.empty((N, H, W, K, 3), dtype=F32, device=dev)
+    positions = torch.empty((N, H, W, K, 3), dtype=F32, device=dev) if return_positions else None
+    if colors.numel() == 0:
+        return colors, positions
+    _launch(dev, "shading_forward", _ptr(p2f), _ptr(bary), _ptr(fp), _ptr(fn), F, _ptr(tx), _ptr(prm), N, H, W, K,
+            int(bool(flat)), LIGHT_KINDS[light], _ptr(colors), _ptr(positions))
     return colors, positions
+
+
+def _outputs(dev, *wanted):
+    """float32 tensors of the (flag, shape) pairs `wanted`, None where the flag is false."""
+    return [torch.empty(shape, dtype=F32, device=dev) if flag else None for flag, shape in wanted]
 
 
 def shading_backward(grad_colors: torch.Tensor, grad_positions, pix_to_face: torch.Tensor, barycentric_coords,
@@ -773,80 +779,56 @@ def shading_backward(grad_colors: torch.Tensor, grad_positions, pix_to_face: tor
     """Backward of `shading_forward` -> (grad_texels, grad_barycentric_coords, grad_face_positions, grad_face_normals,
     grad_params); an entry is None where `needs_input_grad` (same order) is false, and grad_barycentric_coords is None
     in flat mode.  grad_params is deterministic; the two face gradients are accumulated with atomics."""
-    dev = _check_shading_inputs(pix_to_face, barycentric_coords, face_positions, face_normals, texels, params, flat,
-                                light)
-    shape = tuple(pix_to_face.shape) + (3,)
-    for name, t in (("grad_colors", grad_colors), ("grad_positions", grad_positions)):
-        if t is not None:
-            _require_cuda((name, t), ("pix_to_face", pix_to_face))
-            if t.dtype != torch.float32 or tuple(t.shape) != shape:
-                raise RuntimeError("%s must be a float32 tensor of shape (N, H, W, K, 3)" % name)
-    lib = _lib.load()
-    N, H, W, K = (int(v) for v in pix_to_face.shape)
-    F = int(face_positions.shape[0])
+    N, H, W, K, F, dev = _check_shading_inputs(pix_to_face, barycentric_coords, face_positions, face_normals, texels,
+                                               params, flat, light,
+                                               (("grad_colors", grad_colors), ("grad_positions", grad_positions)))
+    shape = (N, H, W, K, 3)
     need_tx, need_bary, need_fp, need_fn, need_prm = (bool(v) for v in needs_input_grad)
     need_bary = need_bary and not flat
     need_fn = need_fn and face_normals is not None
     gc, p2f, tx, prm = grad_colors.contiguous(), pix_to_face.contiguous(), texels.contiguous(), params.contiguous()
-    gp = None if grad_positions is None else grad_positions.contiguous()
-    fp = face_positions.contiguous()
+    gp, fp = _c(grad_positions), face_positions.contiguous()
     bary = None if flat else barycentric_coords.contiguous()
     fn = None if light == "ambient" else face_normals.contiguous()
-    with torch.cuda.device(dev):
-        def out(flag, like_shape):
-            return torch.empty(like_shape, dtype=torch.float32, device=dev) if flag else None
-        g_tx, g_bary = out(need_tx, shape), out(need_bary, shape)
-        g_fp = out(need_fp, tuple(face_positions.shape))
-        g_fn = out(need_fn, tuple(face_normals.shape)) if need_fn else None
-        g_prm = out(need_prm, (N, SHADING_PARAMS))
-        ws_bytes = int(lib.b200r_shading_workspace_bytes(N, H, W, K)) if need_prm else 0
-        ws = torch.empty((ws_bytes // 4,), dtype=torch.float32, device=dev) if ws_bytes else None
-        _lib.check(lib.b200r_shading_backward(
-            _ptr(gc), _ptr(gp), _ptr(p2f), _ptr(bary), _ptr(fp), _ptr(fn), F, _ptr(tx), _ptr(prm), N, H, W, K,
-            int(bool(flat)), LIGHT_KINDS[light], _ptr(ws), ws_bytes, _ptr(g_tx), _ptr(g_bary), _ptr(g_fp), _ptr(g_fn),
-            _ptr(g_prm), _stream_ptr(dev)))
-        if N * H * W * K == 0:  # nothing was launched: the outputs the kernels would have written
-            for t in (g_tx, g_bary):
-                if t is not None:
-                    t.zero_()
+    g_tx, g_bary, g_fp, g_fn, g_prm = _outputs(
+        dev, (need_tx, shape), (need_bary, shape), (need_fp, tuple(face_positions.shape)),
+        (need_fn, tuple(face_normals.shape) if need_fn else None), (need_prm, (N, SHADING_PARAMS)))
+    ws, ws_bytes = _workspace(dev, "shading", N, H, W, K) if need_prm else (None, 0)
+    _launch(dev, "shading_backward", _ptr(gc), _ptr(gp), _ptr(p2f), _ptr(bary), _ptr(fp), _ptr(fn), F, _ptr(tx),
+            _ptr(prm), N, H, W, K, int(bool(flat)), LIGHT_KINDS[light], _ptr(ws), ws_bytes, _ptr(g_tx), _ptr(g_bary),
+            _ptr(g_fp), _ptr(g_fn), _ptr(g_prm))
+    if N * H * W * K == 0:  # nothing was launched: the outputs the kernels would have written
+        for t in (g_tx, g_bary):
+            if t is not None:
+                t.zero_()
     return g_tx, g_bary, g_fp, g_fn, g_prm
 
 
 def _check_gouraud_inputs(verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params, faces, pix_to_face,
-                          barycentric_coords, light):
-    """The device; raises RuntimeError naming the argument for anything the kernels cannot take."""
+                          barycentric_coords, light, grads=()):
+    """(V, F, meshes, device); raises RuntimeError naming the argument for anything the kernels cannot take.  `grads`
+    are the backward's (name, tensor, shape, dims) extra float32 inputs."""
     if light not in LIGHT_KINDS:
         raise RuntimeError("light must be one of %s, got %r" % (sorted(LIGHT_KINDS), light))
     if light != "ambient" and normals is None:
         raise RuntimeError("normals are required for %s light" % light)
     floats = [("verts", verts), ("verts_colors", verts_colors), ("params", params),
-              ("barycentric_coords", barycentric_coords)]
-    if normals is not None:
-        floats.append(("normals", normals))
-    dev = _check_blend_inputs(floats, pix_to_face)
-    _require_cuda(("faces", faces), ("mesh_first_vert", mesh_first_vert), ("mesh_num_verts", mesh_num_verts),
-                  ("pix_to_face", pix_to_face))
-    V = int(verts.shape[0]) if verts.dim() == 2 else -1
-    for name, t in floats:
-        if name in ("verts", "verts_colors", "normals") and (t.dim() != 2 or tuple(t.shape) != (V, 3)):
-            raise RuntimeError("%s must be (V, 3) with the V of verts, got %s" % (name, tuple(t.shape)))
-    for name, t in (("faces", faces), ("mesh_first_vert", mesh_first_vert), ("mesh_num_verts", mesh_num_verts)):
-        if t.dtype != torch.int64:
-            raise RuntimeError("expected scalar type Long but found %s for %s" % (t.dtype, name))
-    if faces.dim() != 2 or faces.shape[1] != 3:
-        raise RuntimeError("faces must be (F, 3), got %s" % (tuple(faces.shape),))
-    meshes = int(mesh_first_vert.shape[0]) if mesh_first_vert.dim() == 1 else -1
-    if meshes < 0 or tuple(mesh_num_verts.shape) != (meshes,):
-        raise RuntimeError("mesh_first_vert and mesh_num_verts must be (meshes,), got %s and %s"
-                           % (tuple(mesh_first_vert.shape), tuple(mesh_num_verts.shape)))
+              ("barycentric_coords", barycentric_coords)] + ([("normals", normals)] if normals is not None else [])
+    V, F, dev = _check_verts_faces(None, verts, faces, *[g[:2] for g in grads], *floats[1:],
+                                   ("mesh_first_vert", mesh_first_vert), ("mesh_num_verts", mesh_num_verts),
+                                   ("pix_to_face", pix_to_face))
+    for name, t in (("verts_colors", verts_colors), ("normals", normals)):
+        if t is not None:
+            _check_float(name, t, (V, 3), "V, 3")
+    meshes = _check_ranges(None, "mesh_first_vert", mesh_first_vert, "mesh_num_verts", mesh_num_verts)
     if meshes > 65535:
         raise RuntimeError("at most 65535 meshes per call, got %d" % meshes)
-    if tuple(params.shape) != (meshes, SHADING_PARAMS):
-        raise RuntimeError("params must be (meshes, %d), got %s" % (SHADING_PARAMS, tuple(params.shape)))
-    if tuple(barycentric_coords.shape) != tuple(pix_to_face.shape) + (3,):
-        raise RuntimeError("barycentric_coords must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
-                           % (tuple(barycentric_coords.shape),))
-    return dev
+    _check_float("params", params, (meshes, SHADING_PARAMS), "meshes, %d" % SHADING_PARAMS)
+    shape = _check_index(pix_to_face)
+    _check_float("barycentric_coords", barycentric_coords, shape + (3,), "N, H, W, K, 3")
+    for name, t, g_shape, dims in grads:
+        _check_float(name, t, g_shape, dims)
+    return V, F, meshes, dev
 
 
 def gouraud_forward(verts: torch.Tensor, normals, verts_colors: torch.Tensor, mesh_first_vert: torch.Tensor,
@@ -856,21 +838,17 @@ def gouraud_forward(verts: torch.Tensor, normals, verts_colors: torch.Tensor, me
     light), verts_colors (V,3) f32 packed; mesh_first_vert, mesh_num_verts (meshes,) i64; params (meshes,22) f32, one
     row per mesh; faces (F,3) i64 packed; pix_to_face (N,H,W,K) i64; barycentric_coords (N,H,W,K,3) f32; light
     "point", "directional" or "ambient".  -> (colors (N,H,W,K,3), verts_shaded (V,3))."""
-    dev = _check_gouraud_inputs(verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params, faces,
-                                pix_to_face, barycentric_coords, light)
-    lib = _lib.load()
-    V, F, meshes = int(verts.shape[0]), int(faces.shape[0]), int(mesh_first_vert.shape[0])
+    V, F, meshes, dev = _check_gouraud_inputs(verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params,
+                                              faces, pix_to_face, barycentric_coords, light)
     P = pix_to_face.numel()
     v, vc, prm, fc = verts.contiguous(), verts_colors.contiguous(), params.contiguous(), faces.contiguous()
     nrm = None if light == "ambient" else normals.contiguous()
     first, num = mesh_first_vert.contiguous(), mesh_num_verts.contiguous()
     p2f, bary = pix_to_face.contiguous(), barycentric_coords.contiguous()
-    with torch.cuda.device(dev):
-        shaded = torch.empty((V, 3), dtype=torch.float32, device=dev)
-        colors = torch.empty(tuple(pix_to_face.shape) + (3,), dtype=torch.float32, device=dev)
-        _lib.check(lib.b200r_gouraud_forward(_ptr(v), _ptr(nrm), _ptr(vc), V, _ptr(first), _ptr(num), meshes,
-                                             _ptr(prm), _ptr(fc), F, _ptr(p2f), _ptr(bary), P, LIGHT_KINDS[light],
-                                             _ptr(shaded), _ptr(colors), _stream_ptr(dev)))
+    shaded = torch.empty((V, 3), dtype=F32, device=dev)
+    colors = torch.empty(tuple(pix_to_face.shape) + (3,), dtype=F32, device=dev)
+    _launch(dev, "gouraud_forward", _ptr(v), _ptr(nrm), _ptr(vc), V, _ptr(first), _ptr(num), meshes, _ptr(prm),
+            _ptr(fc), F, _ptr(p2f), _ptr(bary), P, LIGHT_KINDS[light], _ptr(shaded), _ptr(colors))
     return colors, shaded
 
 
@@ -882,38 +860,28 @@ def gouraud_backward(grad_colors: torch.Tensor, verts: torch.Tensor, normals, ve
     grad_params); an entry is None where `needs_input_grad` (same order) is false.  grad_barycentric_coords is
     deterministic; the other four start from a per-vertex sum accumulated with atomics, so requesting them under
     torch.use_deterministic_algorithms(True) raises, as the reference's interpolation backward does."""
-    dev = _check_gouraud_inputs(verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params, faces,
-                                pix_to_face, barycentric_coords, light)
-    _require_cuda(("grad_colors", grad_colors), ("verts_shaded", verts_shaded), ("pix_to_face", pix_to_face))
-    if grad_colors.dtype != torch.float32 or tuple(grad_colors.shape) != tuple(pix_to_face.shape) + (3,):
-        raise RuntimeError("grad_colors must be a float32 tensor of shape (N, H, W, K, 3)")
-    if verts_shaded.dtype != torch.float32 or tuple(verts_shaded.shape) != tuple(verts.shape):
-        raise RuntimeError("verts_shaded must be a float32 tensor of shape (V, 3)")
+    grads = (("grad_colors", grad_colors, tuple(pix_to_face.shape) + (3,), "N, H, W, K, 3"),
+             ("verts_shaded", verts_shaded, tuple(verts.shape), "V, 3"))
+    V, F, meshes, dev = _check_gouraud_inputs(verts, normals, verts_colors, mesh_first_vert, mesh_num_verts, params,
+                                              faces, pix_to_face, barycentric_coords, light, grads)
     need_v, need_n, need_vc, need_bary, need_prm = (bool(x) for x in needs_input_grad)
     need_n = need_n and normals is not None
-    if ((need_v or need_n or need_vc or need_prm) and torch.are_deterministic_algorithms_enabled()
-            and not torch.is_deterministic_algorithms_warn_only_enabled()):
-        raise RuntimeError(
-            "gouraud_backward does not have a deterministic implementation (the gradient of the shaded vertex colours "
-            "is accumulated with atomics), but you set 'torch.use_deterministic_algorithms(True)'.")
-    lib = _lib.load()
-    V, F, meshes = int(verts.shape[0]), int(faces.shape[0]), int(mesh_first_vert.shape[0])
+    need_vertex = need_v or need_n or need_vc or need_prm
+    if need_vertex:
+        _refuse_nondeterministic("gouraud_backward",
+                                 "the gradient of the shaded vertex colours is accumulated with atomics")
     P = pix_to_face.numel()
     gc, v, vc, prm = grad_colors.contiguous(), verts.contiguous(), verts_colors.contiguous(), params.contiguous()
     nrm = None if light == "ambient" else normals.contiguous()
     first, num, fc = mesh_first_vert.contiguous(), mesh_num_verts.contiguous(), faces.contiguous()
     p2f, bary, shaded = pix_to_face.contiguous(), barycentric_coords.contiguous(), verts_shaded.contiguous()
-    with torch.cuda.device(dev):
-        def out(flag, shape):
-            return torch.empty(shape, dtype=torch.float32, device=dev) if flag else None
-        g_v, g_n, g_vc = out(need_v, (V, 3)), out(need_n, (V, 3)), out(need_vc, (V, 3))
-        g_bary, g_prm = out(need_bary, tuple(barycentric_coords.shape)), out(need_prm, (meshes, SHADING_PARAMS))
-        ws_bytes = int(lib.b200r_gouraud_workspace_bytes(meshes, V)) if (need_v or need_n or need_vc or need_prm) else 0
-        ws = torch.empty((ws_bytes // 4,), dtype=torch.float32, device=dev) if ws_bytes else None
-        _lib.check(lib.b200r_gouraud_backward(
-            _ptr(gc), _ptr(v), _ptr(nrm), _ptr(vc), V, _ptr(first), _ptr(num), meshes, _ptr(prm), _ptr(fc), F,
-            _ptr(p2f), _ptr(bary), P, LIGHT_KINDS[light], _ptr(shaded), _ptr(ws), ws_bytes, _ptr(g_v), _ptr(g_n),
-            _ptr(g_vc), _ptr(g_bary), _ptr(g_prm), _stream_ptr(dev)))
+    g_v, g_n, g_vc, g_bary, g_prm = _outputs(dev, (need_v, (V, 3)), (need_n, (V, 3)), (need_vc, (V, 3)),
+                                             (need_bary, tuple(barycentric_coords.shape)),
+                                             (need_prm, (meshes, SHADING_PARAMS)))
+    ws, ws_bytes = _workspace(dev, "gouraud", meshes, V) if need_vertex else (None, 0)
+    _launch(dev, "gouraud_backward", _ptr(gc), _ptr(v), _ptr(nrm), _ptr(vc), V, _ptr(first), _ptr(num), meshes,
+            _ptr(prm), _ptr(fc), F, _ptr(p2f), _ptr(bary), P, LIGHT_KINDS[light], _ptr(shaded), _ptr(ws), ws_bytes,
+            _ptr(g_v), _ptr(g_n), _ptr(g_vc), _ptr(g_bary), _ptr(g_prm))
     return g_v, g_n, g_vc, g_bary, g_prm
 
 
@@ -921,30 +889,39 @@ SAMPLING_MODES = {"bilinear": 0, "nearest": 1}  # B200R_SAMPLE_*: torch's GridSa
 PADDING_MODES = {"zeros": 0, "border": 1, "reflection": 2}  # B200R_PAD_*: torch's GridSamplerPadding
 
 
-def _check_texture_inputs(pix_to_face, barycentric_coords, face_uvs, maps, sampling_mode, padding_mode):
+def _check_texture_inputs(pix_to_face, barycentric_coords, face_uvs, maps, sampling_mode, padding_mode,
+                          grad_texels=None):
     """(N, H, W, K, H_in, W_in, C, device); raises RuntimeError naming the argument for anything the kernels cannot
-    take, and ValueError when the maps' batch is not the Fragments' N."""
+    take, and ValueError when the maps' batch is not the Fragments' N.  Shapes are checked before devices and dtypes,
+    so that a CPU caller learns about a wrong shape first."""
     if sampling_mode not in SAMPLING_MODES:
         raise RuntimeError("sampling_mode must be one of %s, got %r" % (sorted(SAMPLING_MODES), sampling_mode))
     if padding_mode not in PADDING_MODES:
         raise RuntimeError("padding_mode must be one of %s, got %r" % (sorted(PADDING_MODES), padding_mode))
-    if pix_to_face.dim() != 4:
-        raise RuntimeError("pix_to_face must have dimensions (N, H, W, K)")
-    shape = tuple(pix_to_face.shape)
-    if tuple(barycentric_coords.shape) != shape + (3,):
-        raise RuntimeError("barycentric_coords must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
-                           % (tuple(barycentric_coords.shape),))
-    if face_uvs.dim() != 3 or tuple(face_uvs.shape[1:]) != (3, 2):
-        raise RuntimeError("face_uvs must be (F, 3, 2), got %s" % (tuple(face_uvs.shape),))
-    if maps.dim() != 4 or min(maps.shape[1:]) < 1:
+    shape = _check_index(pix_to_face, dtype=None)
+    _check_tensor("barycentric_coords", barycentric_coords, None, shape + (3,), "N, H, W, K, 3")
+    _check_tensor("face_uvs", face_uvs, None, (None, 3, 2), "F, 3, 2")
+    _check_tensor("maps", maps, None, (None,) * 4, "N, H_in, W_in, C")
+    if min(maps.shape[1:]) < 1:
         raise RuntimeError("maps must be (N, H_in, W_in, C) with H_in, W_in, C >= 1, got %s" % (tuple(maps.shape),))
     if maps.shape[0] != shape[0]:
         raise ValueError("maps must have one map per image: maps has batch %d, the Fragments have N = %d"
                          % (maps.shape[0], shape[0]))
-    dev = _check_blend_inputs([("barycentric_coords", barycentric_coords), ("face_uvs", face_uvs), ("maps", maps)],
-                              pix_to_face)
     H_in, W_in, C = (int(v) for v in maps.shape[1:])
-    return shape + (H_in, W_in, C, dev)
+    floats = [("barycentric_coords", barycentric_coords), ("face_uvs", face_uvs), ("maps", maps)]
+    if grad_texels is not None:
+        _check_tensor("grad_texels", grad_texels, None, shape + (C,), "N, H, W, K, C")
+        floats.insert(0, ("grad_texels", grad_texels))
+    return shape + (H_in, W_in, C, _check_texture_devices(pix_to_face, floats))
+
+
+def _check_texture_devices(pix_to_face, floats):
+    """The device of pix_to_face and the (name, tensor) `floats`, after their shapes: then their dtypes."""
+    dev = _require_cuda(*floats, ("pix_to_face", pix_to_face))
+    _check_tensor("pix_to_face", pix_to_face, I64)
+    for name, t in floats:
+        _check_float(name, t)
+    return dev
 
 
 def texture_uv_forward(pix_to_face: torch.Tensor, barycentric_coords: torch.Tensor, face_uvs: torch.Tensor,
@@ -955,16 +932,13 @@ def texture_uv_forward(pix_to_face: torch.Tensor, barycentric_coords: torch.Tens
     (channel last, read in place when contiguous) -> texels (N,H,W,K,C) f32, contiguous."""
     N, H, W, K, H_in, W_in, C, dev = _check_texture_inputs(pix_to_face, barycentric_coords, face_uvs, maps,
                                                            sampling_mode, padding_mode)
-    lib = _lib.load()
     F = int(face_uvs.shape[0])
     p2f, bary, fuv, m = pix_to_face.contiguous(), barycentric_coords.contiguous(), face_uvs.contiguous(), maps.contiguous()
-    with torch.cuda.device(dev):
-        texels = torch.empty((N, H, W, K, C), dtype=torch.float32, device=dev)
-        if texels.numel() == 0:
-            return texels
-        _lib.check(lib.b200r_texture_uv_forward(_ptr(p2f), _ptr(bary), _ptr(fuv), F, _ptr(m), N, H, W, K, H_in, W_in,
-                                                C, SAMPLING_MODES[sampling_mode], PADDING_MODES[padding_mode],
-                                                int(bool(align_corners)), _ptr(texels), _stream_ptr(dev)))
+    texels = torch.empty((N, H, W, K, C), dtype=F32, device=dev)
+    if texels.numel() == 0:
+        return texels
+    _launch(dev, "texture_uv_forward", _ptr(p2f), _ptr(bary), _ptr(fuv), F, _ptr(m), N, H, W, K, H_in, W_in, C,
+            SAMPLING_MODES[sampling_mode], PADDING_MODES[padding_mode], int(bool(align_corners)), _ptr(texels))
     return texels
 
 
@@ -976,29 +950,18 @@ def texture_uv_backward(grad_texels: torch.Tensor, pix_to_face: torch.Tensor, ba
     deterministic; the other two are accumulated with atomics, so requesting them under
     torch.use_deterministic_algorithms(True) raises, as torch's grid sampler backward does."""
     N, H, W, K, H_in, W_in, C, dev = _check_texture_inputs(pix_to_face, barycentric_coords, face_uvs, maps,
-                                                           sampling_mode, padding_mode)
-    _require_cuda(("grad_texels", grad_texels), ("pix_to_face", pix_to_face))
-    if grad_texels.dtype != torch.float32 or tuple(grad_texels.shape) != (N, H, W, K, C):
-        raise RuntimeError("grad_texels must be a float32 tensor of shape (N, H, W, K, C) = %s, got %s %s"
-                           % ((N, H, W, K, C), grad_texels.dtype, tuple(grad_texels.shape)))
+                                                           sampling_mode, padding_mode, grad_texels)
     need_maps, need_bary, need_fuv = (bool(v) for v in needs_input_grad)
-    if ((need_maps or need_fuv) and torch.are_deterministic_algorithms_enabled()
-            and not torch.is_deterministic_algorithms_warn_only_enabled()):
-        raise RuntimeError(
-            "texture_uv_backward does not have a deterministic implementation (grad_maps and grad_face_uvs are "
-            "accumulated with atomics), but you set 'torch.use_deterministic_algorithms(True)'.")
-    lib = _lib.load()
+    if need_maps or need_fuv:
+        _refuse_nondeterministic("texture_uv_backward", "grad_maps and grad_face_uvs are accumulated with atomics")
     F = int(face_uvs.shape[0])
     go = grad_texels.contiguous()
     p2f, bary, fuv, m = pix_to_face.contiguous(), barycentric_coords.contiguous(), face_uvs.contiguous(), maps.contiguous()
-    with torch.cuda.device(dev):
-        g_maps = torch.empty((N, H_in, W_in, C), dtype=torch.float32, device=dev) if need_maps else None
-        g_bary = torch.empty((N, H, W, K, 3), dtype=torch.float32, device=dev) if need_bary else None
-        g_fuv = torch.empty((F, 3, 2), dtype=torch.float32, device=dev) if need_fuv else None
-        _lib.check(lib.b200r_texture_uv_backward(
-            _ptr(go), _ptr(p2f), _ptr(bary), _ptr(fuv), F, _ptr(m), N, H, W, K, H_in, W_in, C,
-            SAMPLING_MODES[sampling_mode], PADDING_MODES[padding_mode], int(bool(align_corners)), _ptr(g_maps),
-            _ptr(g_bary), _ptr(g_fuv), _stream_ptr(dev)))
+    g_maps, g_bary, g_fuv = _outputs(dev, (need_maps, (N, H_in, W_in, C)), (need_bary, (N, H, W, K, 3)),
+                                     (need_fuv, (F, 3, 2)))
+    _launch(dev, "texture_uv_backward", _ptr(go), _ptr(p2f), _ptr(bary), _ptr(fuv), F, _ptr(m), N, H, W, K, H_in, W_in,
+            C, SAMPLING_MODES[sampling_mode], PADDING_MODES[padding_mode], int(bool(align_corners)), _ptr(g_maps),
+            _ptr(g_bary), _ptr(g_fuv))
     return g_maps, g_bary, g_fuv
 
 
@@ -1009,19 +972,20 @@ def texture_atlas_key_bits(F: int, R: int):
     return bits, 4 if bits <= 32 else 8
 
 
-def _check_atlas_inputs(pix_to_face, barycentric_coords, atlas):
-    """(N, H, W, K, F, R, C, device); raises RuntimeError naming the argument for anything the kernels cannot take."""
-    if pix_to_face.dim() != 4:
-        raise RuntimeError("pix_to_face must have dimensions (N, H, W, K)")
-    shape = tuple(pix_to_face.shape)
-    if tuple(barycentric_coords.shape) != shape + (3,):
-        raise RuntimeError("barycentric_coords must be (N, H, W, K, 3) with the (N, H, W, K) of pix_to_face, got %s"
-                           % (tuple(barycentric_coords.shape),))
-    if atlas.dim() != 4 or atlas.shape[1] != atlas.shape[2] or atlas.shape[1] < 1 or atlas.shape[3] < 1:
+def _check_atlas_inputs(pix_to_face, barycentric_coords, atlas, grad_texels=None):
+    """(N, H, W, K, F, R, C, device); raises RuntimeError naming the argument for anything the kernels cannot take.
+    Shapes are checked before devices and dtypes, as for the UV textures."""
+    shape = _check_index(pix_to_face, dtype=None)
+    _check_tensor("barycentric_coords", barycentric_coords, None, shape + (3,), "N, H, W, K, 3")
+    _check_tensor("atlas", atlas, None, (None,) * 4, "F, R, R, C")
+    if atlas.shape[1] != atlas.shape[2] or atlas.shape[1] < 1 or atlas.shape[3] < 1:
         raise RuntimeError("atlas must be (F, R, R, C) with R, C >= 1, got %s" % (tuple(atlas.shape),))
-    dev = _check_blend_inputs([("barycentric_coords", barycentric_coords), ("atlas", atlas)], pix_to_face)
     F, R, _, C = (int(v) for v in atlas.shape)
-    return shape + (F, R, C, dev)
+    floats = [("barycentric_coords", barycentric_coords), ("atlas", atlas)]
+    if grad_texels is not None:
+        _check_tensor("grad_texels", grad_texels, None, shape + (C,), "N, H, W, K, C")
+        floats.insert(0, ("grad_texels", grad_texels))
+    return shape + (F, R, C, _check_texture_devices(pix_to_face, floats))
 
 
 def texture_atlas_forward(pix_to_face: torch.Tensor, barycentric_coords: torch.Tensor, atlas: torch.Tensor):
@@ -1029,14 +993,11 @@ def texture_atlas_forward(pix_to_face: torch.Tensor, barycentric_coords: torch.T
     (N,H,W,K) i64, barycentric_coords (N,H,W,K,3) f32, atlas (F,R,R,C) f32, the packed atlas (read in place when
     contiguous) -> texels (N,H,W,K,C) f32, contiguous.  Slots whose cell the reference cannot index (it raises) get 0."""
     N, H, W, K, F, R, C, dev = _check_atlas_inputs(pix_to_face, barycentric_coords, atlas)
-    lib = _lib.load()
     p2f, bary, a = pix_to_face.contiguous(), barycentric_coords.contiguous(), atlas.contiguous()
-    with torch.cuda.device(dev):
-        texels = torch.empty((N, H, W, K, C), dtype=torch.float32, device=dev)
-        if texels.numel() == 0:
-            return texels
-        _lib.check(lib.b200r_texture_atlas_forward(_ptr(p2f), _ptr(bary), _ptr(a), F, R, C, N, H, W, K, _ptr(texels),
-                                                   _stream_ptr(dev)))
+    texels = torch.empty((N, H, W, K, C), dtype=F32, device=dev)
+    if texels.numel() == 0:
+        return texels
+    _launch(dev, "texture_atlas_forward", _ptr(p2f), _ptr(bary), _ptr(a), F, R, C, N, H, W, K, _ptr(texels))
     return texels
 
 
@@ -1045,19 +1006,12 @@ def texture_atlas_backward(grad_texels: torch.Tensor, pix_to_face: torch.Tensor,
     """Backward of `texture_atlas_forward` -> grad_atlas (F,R,R,C) f32: each cell's sum of grad_texels ·
     float(pix_to_face >= 0) over the slots that read it, in ascending slot order.  Deterministic (a stable sort, no
     atomics), so it runs under torch.use_deterministic_algorithms(True); nothing synchronises the host."""
-    N, H, W, K, F, R, C, dev = _check_atlas_inputs(pix_to_face, barycentric_coords, atlas)
-    _require_cuda(("grad_texels", grad_texels), ("pix_to_face", pix_to_face))
-    if grad_texels.dtype != torch.float32 or tuple(grad_texels.shape) != (N, H, W, K, C):
-        raise RuntimeError("grad_texels must be a float32 tensor of shape (N, H, W, K, C) = %s, got %s %s"
-                           % ((N, H, W, K, C), grad_texels.dtype, tuple(grad_texels.shape)))
-    lib = _lib.load()
+    N, H, W, K, F, R, C, dev = _check_atlas_inputs(pix_to_face, barycentric_coords, atlas, grad_texels)
     go, p2f, bary = grad_texels.contiguous(), pix_to_face.contiguous(), barycentric_coords.contiguous()
-    with torch.cuda.device(dev):
-        grad_atlas = torch.empty((F, R, R, C), dtype=torch.float32, device=dev)
-        ws_bytes = int(lib.b200r_texture_atlas_workspace_bytes(N, H, W, K, F, R))
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None  # 512-byte aligned
-        _lib.check(lib.b200r_texture_atlas_backward(_ptr(go), _ptr(p2f), _ptr(bary), F, R, C, N, H, W, K, _ptr(ws),
-                                                    ws_bytes, _ptr(grad_atlas), _stream_ptr(dev)))
+    grad_atlas = torch.empty((F, R, R, C), dtype=F32, device=dev)
+    ws, ws_bytes = _workspace(dev, "texture_atlas", N, H, W, K, F, R)
+    _launch(dev, "texture_atlas_backward", _ptr(go), _ptr(p2f), _ptr(bary), F, R, C, N, H, W, K, _ptr(ws), ws_bytes,
+            _ptr(grad_atlas))
     return grad_atlas
 
 
@@ -1072,52 +1026,29 @@ def normals_table_size(V: int, F: int):
     return int(V) + 1 + 3 * int(F)
 
 
-def _check_mesh_inputs(op, verts, faces):
-    """(V, F, device) of float32 verts (V, 3) and int64 faces (F, 3) on one CUDA device; raises RuntimeError otherwise,
-    and for sizes past the kernels' limits (V < 2^31 - 1, 3F < 2^31)."""
-    dev = _require_cuda(("verts", verts), ("faces", faces))
-    if verts.dtype != torch.float32:
-        raise RuntimeError("%s: expected scalar type Float for verts but found %s" % (op, verts.dtype))
-    if faces.dtype != torch.int64:
-        raise RuntimeError("%s: expected scalar type Long for faces but found %s" % (op, faces.dtype))
-    if verts.dim() != 2 or verts.shape[1] != 3:
-        raise RuntimeError("%s: verts must be (V, 3), got %s" % (op, tuple(verts.shape)))
-    if faces.dim() != 2 or faces.shape[1] != 3:
-        raise RuntimeError("%s: faces must be (F, 3), got %s" % (op, tuple(faces.shape)))
-    V, F = int(verts.shape[0]), int(faces.shape[0])
-    if V >= (1 << 31) - 1 or 3 * F >= (1 << 31):
+def normals_sizes_ok(V: int, F: int):
+    """Whether the normal kernels take these sizes (b200r_normals_workspace_bytes)."""
+    return V < (1 << 31) - 1 and 3 * F < (1 << 31)
+
+
+def _check_normals_inputs(op, verts, faces, *named):
+    """(V, F, device) of verts / faces on one CUDA device with the (name, tensor) pairs `named`, within the kernels'
+    size limits."""
+    V, F, dev = _check_verts_faces(op, verts, faces, *named)
+    if not normals_sizes_ok(V, F):
         raise RuntimeError("%s: at most 2^31 - 2 vertices and (2^31 - 1) / 3 faces, got V = %d, F = %d" % (op, V, F))
     return V, F, dev
-
-
-def _check_grad(name, t, shape, dev):
-    _require_cuda((name, t))
-    if t.device != dev:
-        raise RuntimeError("Expected all tensors to be on the same device (%s is on %s, expected %s)"
-                           % (name, t.device, dev))
-    if t.dtype != torch.float32 or tuple(t.shape) != tuple(shape):
-        raise RuntimeError("%s must be a float32 tensor of shape %s, got %s %s"
-                           % (name, tuple(shape), t.dtype, tuple(t.shape)))
-    return t.contiguous()
-
-
-def _normals_workspace(lib, V, F, dev):
-    ws_bytes = int(lib.b200r_normals_workspace_bytes(V, F))
-    return torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None, ws_bytes  # 512-byte aligned
 
 
 def face_areas_normals_forward(verts: torch.Tensor, faces: torch.Tensor):
     """pytorch3d._C.face_areas_normals_forward (FaceAreasNormalsForward, csrc/face_areas_normals/face_areas_normals.h)
     for float32: verts (V,3) f32, faces (F,3) i64 -> (areas (F,) f32, normals (F,3) f32), bit-identical to the
     reference's CUDA kernel."""
-    V, F, dev = _check_mesh_inputs("face_areas_normals_forward", verts, faces)
-    lib = _lib.load()
+    V, F, dev = _check_normals_inputs("face_areas_normals_forward", verts, faces)
     v, f = verts.contiguous(), faces.contiguous()
-    with torch.cuda.device(dev):
-        areas = torch.empty((F,), dtype=torch.float32, device=dev)
-        normals = torch.empty((F, 3), dtype=torch.float32, device=dev)
-        _lib.check(lib.b200r_face_areas_normals_forward(_ptr(v), V, _ptr(f), F, _ptr(areas), _ptr(normals),
-                                                        _stream_ptr(dev)))
+    areas = torch.empty((F,), dtype=F32, device=dev)
+    normals = torch.empty((F, 3), dtype=F32, device=dev)
+    _launch(dev, "face_areas_normals_forward", _ptr(v), V, _ptr(f), F, _ptr(areas), _ptr(normals))
     return areas, normals
 
 
@@ -1126,16 +1057,15 @@ def face_areas_normals_backward(grad_areas: torch.Tensor, grad_normals: torch.Te
     """pytorch3d._C.face_areas_normals_backward (FaceAreasNormalsBackward) for float32 -> grad_verts (V,3) f32: the
     reference's per-corner gradients, summed per vertex in a fixed order.  Deterministic (no atomics), so unlike the
     reference it runs under torch.use_deterministic_algorithms(True)."""
-    V, F, dev = _check_mesh_inputs("face_areas_normals_backward", verts, faces)
-    ga = _check_grad("grad_areas", grad_areas, (F,), dev)
-    gn = _check_grad("grad_normals", grad_normals, (F, 3), dev)
-    lib = _lib.load()
-    v, f = verts.contiguous(), faces.contiguous()
-    with torch.cuda.device(dev):
-        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
-        ws, ws_bytes = _normals_workspace(lib, V, F, dev)
-        _lib.check(lib.b200r_face_areas_normals_backward(_ptr(ga), _ptr(gn), _ptr(v), V, _ptr(f), F, _ptr(ws),
-                                                         ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
+    op = "face_areas_normals_backward"
+    V, F, dev = _check_normals_inputs(op, verts, faces, ("grad_areas", grad_areas), ("grad_normals", grad_normals))
+    _check_tensor("grad_areas", grad_areas, F32, (F,), "F,", op)
+    _check_tensor("grad_normals", grad_normals, F32, (F, 3), "F, 3", op)
+    ga, gn, v, f = grad_areas.contiguous(), grad_normals.contiguous(), verts.contiguous(), faces.contiguous()
+    grad_verts = torch.empty((V, 3), dtype=F32, device=dev)
+    ws, ws_bytes = _workspace(dev, "normals", V, F)
+    _launch(dev, "face_areas_normals_backward", _ptr(ga), _ptr(gn), _ptr(v), V, _ptr(f), F, _ptr(ws), ws_bytes,
+            _ptr(grad_verts))
     return grad_verts
 
 
@@ -1144,16 +1074,14 @@ def verts_normals_forward(verts: torch.Tensor, faces: torch.Tensor):
     faces (F,3) i64 -> (normals (V,3) f32, table (V + 1 + 3F,) i32, sums (V,3) f32).  The normals are bit-identical to
     the reference's torch chain on the CPU; the table and the unnormalised sums are what `verts_normals_backward`
     reads."""
-    V, F, dev = _check_mesh_inputs("verts_normals_forward", verts, faces)
-    lib = _lib.load()
+    V, F, dev = _check_normals_inputs("verts_normals_forward", verts, faces)
     v, f = verts.contiguous(), faces.contiguous()
-    with torch.cuda.device(dev):
-        normals = torch.empty((V, 3), dtype=torch.float32, device=dev)
-        table = torch.empty((normals_table_size(V, F),), dtype=torch.int32, device=dev)
-        sums = torch.empty((V, 3), dtype=torch.float32, device=dev)
-        ws, ws_bytes = _normals_workspace(lib, V, F, dev)
-        _lib.check(lib.b200r_verts_normals_forward(_ptr(v), V, _ptr(f), F, _ptr(ws), ws_bytes, _ptr(table),
-                                                   _ptr(sums), _ptr(normals), _stream_ptr(dev)))
+    normals = torch.empty((V, 3), dtype=F32, device=dev)
+    table = torch.empty((normals_table_size(V, F),), dtype=I32, device=dev)
+    sums = torch.empty((V, 3), dtype=F32, device=dev)
+    ws, ws_bytes = _workspace(dev, "normals", V, F)
+    _launch(dev, "verts_normals_forward", _ptr(v), V, _ptr(f), F, _ptr(ws), ws_bytes, _ptr(table), _ptr(sums),
+            _ptr(normals))
     return normals, table, sums
 
 
@@ -1161,19 +1089,17 @@ def verts_normals_backward(grad_normals: torch.Tensor, verts: torch.Tensor, face
                            sums: torch.Tensor):
     """Backward of `verts_normals_forward` -> grad_verts (V,3) f32, from the forward's table and sums (no sort).
     Deterministic, no atomics; nothing synchronises the host."""
-    V, F, dev = _check_mesh_inputs("verts_normals_backward", verts, faces)
-    gn = _check_grad("grad_normals", grad_normals, (V, 3), dev)
-    s = _check_grad("sums", sums, (V, 3), dev)
-    _require_cuda(("table", table))
-    if table.device != dev or table.dtype != torch.int32 or tuple(table.shape) != (normals_table_size(V, F),):
-        raise RuntimeError("table must be the int32 (V + 1 + 3F,) table of verts_normals_forward on %s" % dev)
-    lib = _lib.load()
-    v, f, t = verts.contiguous(), faces.contiguous(), table.contiguous()
-    with torch.cuda.device(dev):
-        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
-        ws, ws_bytes = _normals_workspace(lib, V, F, dev)
-        _lib.check(lib.b200r_verts_normals_backward(_ptr(gn), _ptr(v), V, _ptr(f), F, _ptr(t), _ptr(s), _ptr(ws),
-                                                    ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
+    op = "verts_normals_backward"
+    V, F, dev = _check_normals_inputs(op, verts, faces, ("grad_normals", grad_normals), ("sums", sums),
+                                      ("table", table))
+    _check_tensor("grad_normals", grad_normals, F32, (V, 3), "V, 3", op)
+    _check_tensor("sums", sums, F32, (V, 3), "V, 3", op)
+    _check_tensor("table", table, I32, (normals_table_size(V, F),), "V + 1 + 3F,", op)
+    gn, v, f, t, s = (x.contiguous() for x in (grad_normals, verts, faces, table, sums))
+    grad_verts = torch.empty((V, 3), dtype=F32, device=dev)
+    ws, ws_bytes = _workspace(dev, "normals", V, F)
+    _launch(dev, "verts_normals_backward", _ptr(gn), _ptr(v), V, _ptr(f), F, _ptr(t), _ptr(s), _ptr(ws), ws_bytes,
+            _ptr(grad_verts))
     return grad_verts
 
 
@@ -1181,43 +1107,9 @@ def verts_normals_backward(grad_normals: torch.Tensor, verts: torch.Tensor, face
 SAMPLE_HAS_VALID, SAMPLE_NONFINITE, SAMPLE_BAD_TOTAL, SAMPLE_HAS_EMPTY = 1, 2, 4, 8
 
 
-def _check_sampling_inputs(op, verts, faces, mesh_first_face, mesh_num_faces, num_samples):
-    """(V, F, N, S, device) of float32 verts (V, 3), int64 faces (F, 3) and the int64 (N,) per-mesh face ranges, all on
-    one CUDA device, N >= 1 and S >= 1; raises RuntimeError otherwise and for sizes past the kernels' limits."""
-    dev = _require_cuda(("verts", verts), ("faces", faces), ("mesh_first_face", mesh_first_face),
-                        ("mesh_num_faces", mesh_num_faces))
-    if verts.dtype != torch.float32:
-        raise RuntimeError("%s: expected scalar type Float for verts but found %s" % (op, verts.dtype))
-    if faces.dtype != torch.int64:
-        raise RuntimeError("%s: expected scalar type Long for faces but found %s" % (op, faces.dtype))
-    if verts.dim() != 2 or verts.shape[1] != 3:
-        raise RuntimeError("%s: verts must be (V, 3), got %s" % (op, tuple(verts.shape)))
-    if faces.dim() != 2 or faces.shape[1] != 3:
-        raise RuntimeError("%s: faces must be (F, 3), got %s" % (op, tuple(faces.shape)))
-    N = int(mesh_first_face.shape[0]) if mesh_first_face.dim() == 1 else -1
-    for name, t in (("mesh_first_face", mesh_first_face), ("mesh_num_faces", mesh_num_faces)):
-        if t.dtype != torch.int64 or t.dim() != 1 or t.shape[0] != N or N < 1:
-            raise RuntimeError("%s: %s must be an int64 (N,) tensor with N >= 1 like mesh_first_face, got %s %s"
-                               % (op, name, t.dtype, tuple(t.shape)))
-    V, F, S = int(verts.shape[0]), int(faces.shape[0]), int(num_samples)
-    if S < 1:
-        raise RuntimeError("%s: num_samples must be at least 1, got %d" % (op, S))
-    if not sampling_sizes_ok(V, F, N, S):
-        raise RuntimeError("%s: at most 2^31 - 2 vertices, 2^31 - 1 meshes and 2^40 samples, got V = %d, F = %d, "
-                           "N = %d, S = %d" % (op, V, F, N, S))
-    return V, F, N, S, dev
-
-
 def sampling_sizes_ok(V: int, F: int, N: int, S: int):
     """Whether the sampling kernels take these sizes (b200r_sample_points_forward)."""
     return V < (1 << 31) - 1 and 1 <= N < (1 << 31) and F // 4096 + N + 1 < (1 << 31) and 1 <= S <= (1 << 40) // N
-
-
-def _sampling_workspace(lib, V, F, N, S, pass_, dev):
-    ws_bytes = int(lib.b200r_sample_points_workspace_bytes(V, F, N, S, pass_))
-    if ws_bytes == 0:
-        raise RuntimeError("sample_points: could not size the workspace (V = %d, F = %d, N = %d, S = %d)" % (V, F, N, S))
-    return torch.empty((ws_bytes,), dtype=torch.uint8, device=dev), ws_bytes  # 512-byte aligned
 
 
 def sample_points_forward(verts: torch.Tensor, faces: torch.Tensor, mesh_first_face: torch.Tensor,
@@ -1234,40 +1126,40 @@ def _sample_points_from_draws(verts: torch.Tensor, faces: torch.Tensor, mesh_fir
                               u: torch.Tensor, v: torch.Tensor):
     """Test hook: `sample_points_forward` with the draws given -- face_idx (N,S) i64 packed faces, u and v (N,S) f32 --
     instead of drawn, so that the outputs can be compared bit for bit with the reference's for the same draws."""
-    if face_idx.dim() != 2:
-        raise RuntimeError("face_idx must be (N, S), got %s" % (tuple(face_idx.shape),))
-    N, S = int(face_idx.shape[0]), int(face_idx.shape[1])
-    for name, t, dt in (("face_idx", face_idx, torch.int64), ("u", u, torch.float32), ("v", v, torch.float32)):
-        _require_cuda((name, t))
-        if t.dtype != dt or tuple(t.shape) != (N, S) or t.device != verts.device:
-            raise RuntimeError("%s must be a %s (N, S) tensor on %s" % (name, dt, verts.device))
-    draws = (face_idx.contiguous(), u.contiguous(), v.contiguous())
-    return _sample_points(verts, faces, mesh_first_face, mesh_num_faces, S, return_normals, None, draws)
+    _check_tensor("face_idx", face_idx, I64, (None, None), "N, S")
+    return _sample_points(verts, faces, mesh_first_face, mesh_num_faces, int(face_idx.shape[1]), return_normals, None,
+                          (face_idx, u, v))
 
 
 def _sample_points(verts, faces, mesh_first_face, mesh_num_faces, num_samples, return_normals, seed, draws):
-    V, F, N, S, dev = _check_sampling_inputs("sample_points_forward", verts, faces, mesh_first_face, mesh_num_faces,
-                                             num_samples)
+    op = "sample_points_forward"
+    extra = [("seed", seed)] if draws is None else list(zip(("face_idx", "u", "v"), draws))
+    V, F, dev = _check_verts_faces(op, verts, faces, ("mesh_first_face", mesh_first_face),
+                                   ("mesh_num_faces", mesh_num_faces), *extra)
+    N = _check_ranges(op, "mesh_first_face", mesh_first_face, "mesh_num_faces", mesh_num_faces)
+    S = int(num_samples)
     if draws is None:
-        _require_cuda(("seed", seed))
-        if seed.dtype != torch.int64 or seed.numel() != 2 or seed.device != dev:
-            raise RuntimeError("seed must be two int64 on %s" % dev)
-        seed = seed.contiguous()
-    lib = _lib.load()
-    v, f = verts.contiguous(), faces.contiguous()
-    first, num = mesh_first_face.contiguous(), mesh_num_faces.contiguous()
-    with torch.cuda.device(dev):
-        samples = torch.empty((N, S, 3), dtype=torch.float32, device=dev)
-        normals = torch.empty((N, S, 3), dtype=torch.float32, device=dev) if return_normals else None
-        face_idx = torch.empty((N, S), dtype=torch.int64, device=dev)
-        bary = torch.empty((N, S, 3), dtype=torch.float32, device=dev)
-        status = torch.empty((1,), dtype=torch.int32, device=dev)
-        ws, ws_bytes = _sampling_workspace(lib, V, F, N, S, 0, dev)
-        d_face, d_u, d_v = draws if draws is not None else (None, None, None)
-        _lib.check(lib.b200r_sample_points_forward(
-            _ptr(v), V, _ptr(f), F, _ptr(first), _ptr(num), N, S, None if seed is None else seed.data_ptr(),
-            _ptr(d_face), _ptr(d_u), _ptr(d_v), ws.data_ptr(), ws_bytes, samples.data_ptr(), _ptr(normals),
-            face_idx.data_ptr(), bary.data_ptr(), status.data_ptr(), _stream_ptr(dev)))
+        _check_tensor("seed", seed.reshape(-1), I64, (2,), "2,", op)
+    else:
+        for name, t, dtype in zip(("face_idx", "u", "v"), draws, (I64, F32, F32)):
+            _check_tensor(name, t, dtype, (N, S), "N, S", op)
+    if S < 1:
+        raise RuntimeError("%s: num_samples must be at least 1, got %d" % (op, S))
+    if not sampling_sizes_ok(V, F, N, S):
+        raise RuntimeError("%s: at most 2^31 - 2 vertices, 1 to 2^31 - 1 meshes and 2^40 samples, got V = %d, F = %d, "
+                           "N = %d, S = %d" % (op, V, F, N, S))
+    v, f, first, num = verts.contiguous(), faces.contiguous(), mesh_first_face.contiguous(), mesh_num_faces.contiguous()
+    sd = _c(seed)
+    d_face, d_u, d_v = (t.contiguous() for t in draws) if draws is not None else (None, None, None)
+    samples = torch.empty((N, S, 3), dtype=F32, device=dev)
+    normals = torch.empty((N, S, 3), dtype=F32, device=dev) if return_normals else None
+    face_idx = torch.empty((N, S), dtype=I64, device=dev)
+    bary = torch.empty((N, S, 3), dtype=F32, device=dev)
+    status = torch.empty((1,), dtype=I32, device=dev)
+    ws, ws_bytes = _workspace(dev, "sample_points", V, F, N, S, 0, required=True)
+    _launch(dev, "sample_points_forward", _ptr(v), V, _ptr(f), F, _ptr(first), _ptr(num), N, S, _ptr(sd), _ptr(d_face),
+            _ptr(d_u), _ptr(d_v), _ptr(ws), ws_bytes, samples.data_ptr(), _ptr(normals), face_idx.data_ptr(),
+            bary.data_ptr(), status.data_ptr())
     return samples, normals, face_idx, bary, status
 
 
@@ -1275,42 +1167,22 @@ def sample_points_backward(grad_samples: torch.Tensor, grad_normals, verts: torc
                            face_idx: torch.Tensor, bary: torch.Tensor):
     """Backward of `sample_points_forward` -> grad_verts (V,3) f32, from the forward's face_idx and bary; grad_normals
     may be None.  Deterministic, no float atomics, no host synchronisation."""
-    if face_idx.dim() != 2:
-        raise RuntimeError("face_idx must be (N, S), got %s" % (tuple(face_idx.shape),))
+    op = "sample_points_backward"
+    grads = [("grad_samples", grad_samples)] + ([("grad_normals", grad_normals)] if grad_normals is not None else [])
+    V, F, dev = _check_verts_faces(op, verts, faces, ("face_idx", face_idx), ("bary", bary), *grads)
+    _check_tensor("face_idx", face_idx, I64, (None, None), "N, S", op)
     N, S = int(face_idx.shape[0]), int(face_idx.shape[1])
-    V, F, dev = _check_mesh_inputs_loose("sample_points_backward", verts, faces)
-    if 3 * N * S >= (1 << 31):
-        raise RuntimeError("sample_points_backward: the backward takes 3 N S < 2^31 sample corners, got N = %d, S = %d"
-                           % (N, S))
-    gs = _check_grad("grad_samples", grad_samples, (N, S, 3), dev)
-    gn = _check_grad("grad_normals", grad_normals, (N, S, 3), dev) if grad_normals is not None else None
-    b = _check_grad("bary", bary, (N, S, 3), dev)
-    _require_cuda(("face_idx", face_idx))
-    if face_idx.dtype != torch.int64 or face_idx.device != dev:
-        raise RuntimeError("face_idx must be the int64 (N, S) face_idx of sample_points_forward on %s" % dev)
-    lib = _lib.load()
-    v, f, fi = verts.contiguous(), faces.contiguous(), face_idx.contiguous()
-    with torch.cuda.device(dev):
-        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
-        ws, ws_bytes = _sampling_workspace(lib, V, F, N, S, 1, dev)
-        _lib.check(lib.b200r_sample_points_backward(_ptr(gs), _ptr(gn), _ptr(v), V, _ptr(f), F, N, S, _ptr(fi),
-                                                    _ptr(b), ws.data_ptr(), ws_bytes, _ptr(grad_verts),
-                                                    _stream_ptr(dev)))
+    for name, t in [("bary", bary)] + grads:
+        _check_tensor(name, t, F32, (N, S, 3), "N, S, 3", op)
+    if V >= (1 << 31) - 1 or 3 * N * S >= (1 << 31):
+        raise RuntimeError("%s: at most 2^31 - 2 vertices and 3 N S < 2^31 sample corners, got V = %d, N = %d, S = %d"
+                           % (op, V, N, S))
+    gs, gn, v, f, fi, b = (_c(t) for t in (grad_samples, grad_normals, verts, faces, face_idx, bary))
+    grad_verts = torch.empty((V, 3), dtype=F32, device=dev)
+    ws, ws_bytes = _workspace(dev, "sample_points", V, F, N, S, 1, required=True)
+    _launch(dev, "sample_points_backward", _ptr(gs), _ptr(gn), _ptr(v), V, _ptr(f), F, N, S, _ptr(fi), _ptr(b),
+            _ptr(ws), ws_bytes, _ptr(grad_verts))
     return grad_verts
-
-
-def _check_mesh_inputs_loose(op, verts, faces):
-    """(V, F, device) of float32 verts (V, 3) and int64 faces (F, 3) on one CUDA device, V < 2^31 - 1."""
-    dev = _require_cuda(("verts", verts), ("faces", faces))
-    if verts.dtype != torch.float32 or verts.dim() != 2 or verts.shape[1] != 3:
-        raise RuntimeError("%s: verts must be a float32 (V, 3) tensor, got %s %s" % (op, verts.dtype,
-                                                                                      tuple(verts.shape)))
-    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
-        raise RuntimeError("%s: faces must be an int64 (F, 3) tensor, got %s %s" % (op, faces.dtype,
-                                                                                    tuple(faces.shape)))
-    if verts.shape[0] >= (1 << 31) - 1:
-        raise RuntimeError("%s: at most 2^31 - 2 vertices, got %d" % (op, verts.shape[0]))
-    return int(verts.shape[0]), int(faces.shape[0]), dev
 
 
 # Reductions and status bits of chamfer_forward (B200R_CHAMFER_*).
@@ -1324,48 +1196,29 @@ def chamfer_sizes_ok(N: int, P1: int, P2: int):
     return N >= 1 and P1 >= 1 and P2 >= 1 and 2 * (N * P1 + N * P2) < (1 << 31)
 
 
-def _chamfer_workspace(lib, N, P1, P2, pass_, dev):
-    ws_bytes = int(lib.b200r_chamfer_workspace_bytes(N, P1, P2, pass_))
-    if ws_bytes == 0:
-        raise RuntimeError("chamfer: could not size the workspace (N = %d, P1 = %d, P2 = %d)" % (N, P1, P2))
-    return torch.empty((ws_bytes,), dtype=torch.uint8, device=dev), ws_bytes
-
-
 def _check_chamfer_inputs(op, x, y, x_lengths, y_lengths, x_normals, y_normals, weights):
     """(N, P1, P2, device): float32 x (N, P1, 3) and y (N, P2, 3), int64 (N,) lengths, float32 normals of the clouds'
     shapes and float32 (N,) weights, all on one CUDA device; raises RuntimeError otherwise."""
-    named = [("x", x), ("y", y)] + [(k, t) for k, t in (("x_lengths", x_lengths), ("y_lengths", y_lengths),
-                                                        ("x_normals", x_normals), ("y_normals", y_normals),
-                                                        ("weights", weights)) if t is not None]
-    dev = _require_cuda(*named)
-    for name, t in named:
-        if t.device != dev:
-            raise RuntimeError("%s: expected all tensors on %s, %s is on %s" % (op, dev, name, t.device))
-    for name, t in (("x", x), ("y", y)):
-        if t.dtype != torch.float32 or t.dim() != 3 or t.shape[2] != 3:
-            raise RuntimeError("%s: %s must be a float32 (N, P, 3) tensor, got %s %s" % (op, name, t.dtype,
-                                                                                       tuple(t.shape)))
-    N, P1, P2 = int(x.shape[0]), int(x.shape[1]), int(y.shape[1])
-    if y.shape[0] != N:
-        raise RuntimeError("%s: x and y must have the same batch size" % op)
-    for name, t, P in (("x_lengths", x_lengths, P1), ("y_lengths", y_lengths, P2)):
-        if t is not None and (t.dtype != torch.int64 or tuple(t.shape) != (N,)):
-            raise RuntimeError("%s: %s must be an int64 (N,) tensor" % (op, name))
+    dev = _require_cuda(*[(k, t) for k, t in (("x", x), ("y", y), ("x_lengths", x_lengths), ("y_lengths", y_lengths),
+                                              ("x_normals", x_normals), ("y_normals", y_normals), ("weights", weights))
+                          if t is not None])
+    _check_tensor("x", x, F32, (None, None, 3), "N, P1, 3", op)
+    N, P1 = int(x.shape[0]), int(x.shape[1])
+    _check_tensor("y", y, F32, (N, None, 3), "N, P2, 3", op)
+    P2 = int(y.shape[1])
     if (x_normals is None) != (y_normals is None):
         raise RuntimeError("%s: give both normals or neither" % op)
-    for name, t, P in (("x_normals", x_normals, P1), ("y_normals", y_normals, P2)):
-        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != (N, P, 3)):
-            raise RuntimeError("%s: %s must be a float32 (%d, %d, 3) tensor" % (op, name, N, P))
-    if weights is not None and (weights.dtype != torch.float32 or tuple(weights.shape) != (N,)):
-        raise RuntimeError("%s: weights must be a float32 (N,) tensor" % op)
+    for name, t, dtype, shape, dims in (("x_lengths", x_lengths, I64, (N,), "N,"),
+                                        ("y_lengths", y_lengths, I64, (N,), "N,"),
+                                        ("x_normals", x_normals, F32, (N, P1, 3), "N, P1, 3"),
+                                        ("y_normals", y_normals, F32, (N, P2, 3), "N, P2, 3"),
+                                        ("weights", weights, F32, (N,), "N,")):
+        if t is not None:
+            _check_tensor(name, t, dtype, shape, dims, op)
     if not chamfer_sizes_ok(N, P1, P2):
         raise RuntimeError("%s: takes N, P1, P2 >= 1 and 2 (N P1 + N P2) < 2^31, got N = %d, P1 = %d, P2 = %d"
                            % (op, N, P1, P2))
     return N, P1, P2, dev
-
-
-def _c(t):
-    return t.contiguous() if t is not None else None
 
 
 def chamfer_forward(x, y, x_lengths, y_lengths, x_normals, y_normals, weights, norm: int, point_reduction,
@@ -1381,33 +1234,30 @@ def chamfer_forward(x, y, x_lengths, y_lengths, x_normals, y_normals, weights, n
     pr, br = CHAMFER_POINT[point_reduction], CHAMFER_BATCH[batch_reduction]
     if pr == 0 and br != 0:
         raise RuntimeError("chamfer_forward: batch_reduction must be None when point_reduction is None")
-    lib = _lib.load()
     x, y, xl, yl, xn, yn, w = (_c(t) for t in (x, y, x_lengths, y_lengths, x_normals, y_normals, weights))
     nrm = xn is not None
-    f32 = dict(dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        dist_x = torch.empty((N, P1), **f32)
-        idx_x = torch.empty((N, P1), dtype=torch.int32, device=dev)
-        dist_y = torch.empty((N, P2), **f32) if not single_directional else None
-        idx_y = torch.empty((N, P2), dtype=torch.int32, device=dev) if not single_directional else None
-        cloud = torch.empty((4 * N + 1,), **f32)
-        argmax = torch.empty((2 * N,), dtype=torch.int32, device=dev)
-        status = torch.empty((1,), dtype=torch.int32, device=dev)
-        if pr == 0:
-            out_x = torch.empty((N, P1), **f32)
-            out_y = torch.empty((N, P2), **f32) if not single_directional else None
-            out_nx = torch.empty((N, P1), **f32) if nrm else None
-            out_ny = torch.empty((N, P2), **f32) if nrm and not single_directional else None
-        else:
-            shape = (N,) if br == 0 else ()
-            out_x, out_y = torch.empty(shape, **f32), None
-            out_nx, out_ny = (torch.empty(shape, **f32) if nrm else None), None
-        ws, ws_bytes = _chamfer_workspace(lib, N, P1, P2, 0, dev)
-        _lib.check(lib.b200r_chamfer_forward(
-            _ptr(x), _ptr(y), N, P1, P2, _ptr(xl), _ptr(yl), _ptr(xn), _ptr(yn), _ptr(w), int(norm), pr, br,
-            int(bool(single_directional)), int(bool(abs_cosine)), ws.data_ptr(), ws_bytes, _ptr(dist_x),
+    f32 = dict(dtype=F32, device=dev)
+    dist_x = torch.empty((N, P1), **f32)
+    idx_x = torch.empty((N, P1), dtype=I32, device=dev)
+    dist_y = torch.empty((N, P2), **f32) if not single_directional else None
+    idx_y = torch.empty((N, P2), dtype=I32, device=dev) if not single_directional else None
+    cloud = torch.empty((4 * N + 1,), **f32)
+    argmax = torch.empty((2 * N,), dtype=I32, device=dev)
+    status = torch.empty((1,), dtype=I32, device=dev)
+    if pr == 0:
+        out_x = torch.empty((N, P1), **f32)
+        out_y = torch.empty((N, P2), **f32) if not single_directional else None
+        out_nx = torch.empty((N, P1), **f32) if nrm else None
+        out_ny = torch.empty((N, P2), **f32) if nrm and not single_directional else None
+    else:
+        shape = (N,) if br == 0 else ()
+        out_x, out_y = torch.empty(shape, **f32), None
+        out_nx, out_ny = (torch.empty(shape, **f32) if nrm else None), None
+    ws, ws_bytes = _workspace(dev, "chamfer", N, P1, P2, 0, required=True)
+    _launch(dev, "chamfer_forward", _ptr(x), _ptr(y), N, P1, P2, _ptr(xl), _ptr(yl), _ptr(xn), _ptr(yn), _ptr(w),
+            int(norm), pr, br, int(bool(single_directional)), int(bool(abs_cosine)), _ptr(ws), ws_bytes, _ptr(dist_x),
             _ptr(idx_x), _ptr(dist_y), _ptr(idx_y), _ptr(cloud), _ptr(argmax), _ptr(out_x), _ptr(out_y),
-            _ptr(out_nx), _ptr(out_ny), _ptr(status), _stream_ptr(dev)))
+            _ptr(out_nx), _ptr(out_ny), _ptr(status))
     return (out_x, out_y, out_nx, out_ny), (dist_x, idx_x, dist_y, idx_y, cloud, argmax), status
 
 
@@ -1417,36 +1267,39 @@ def chamfer_backward(x, y, x_lengths, y_lengths, x_normals, y_normals, weights, 
     """Backward of `chamfer_forward`: grads (g_x, g_y, g_nx, g_ny) are the upstream gradients of its outputs (None
     for an output without one: zeros) -> (grad_x, grad_y, grad_x_normals, grad_y_normals), the pairs asked for by
     need_points / need_normals (None otherwise).  Deterministic, no float atomics, no host synchronisation."""
-    N, P1, P2, dev = _check_chamfer_inputs("chamfer_backward", x, y, x_lengths, y_lengths, x_normals, y_normals,
-                                           weights)
+    op = "chamfer_backward"
+    N, P1, P2, dev = _check_chamfer_inputs(op, x, y, x_lengths, y_lengths, x_normals, y_normals, weights)
     pr, br = CHAMFER_POINT[point_reduction], CHAMFER_BATCH[batch_reduction]
-    dist_x, idx_x, dist_y, idx_y, cloud, argmax = state
+    _, idx_x, _, idx_y, cloud, argmax = state
     nrm = x_normals is not None
     need_normals = need_normals and nrm
     if not (need_points or need_normals):
         return None, None, None, None
-    lib = _lib.load()
-    x, y, xl, yl, xn, yn, w = (_c(t) for t in (x, y, x_lengths, y_lengths, x_normals, y_normals, weights))
     shapes = ((N, P1), (N, P2)) if pr == 0 else ((((N,) if br == 0 else ())),) * 2
+    named = [("idx_x", idx_x, I32, (N, P1)), ("cloud", cloud, F32, (4 * N + 1,)), ("argmax", argmax, I32, (2 * N,))]
+    if not single_directional:
+        named.append(("idx_y", idx_y, I32, (N, P2)))
     g = []
-    for k, t in enumerate(grads):
+    for k, (name, t) in enumerate(zip(("grad_loss_x", "grad_loss_y", "grad_normals_x", "grad_normals_y"), grads)):
         present = (k % 2 == 0 or pr == 0) and (k < 2 or nrm) and not (k % 2 == 1 and single_directional)
         if not present:
             g.append(None)
         elif t is None:
-            g.append(torch.zeros(shapes[k % 2], dtype=torch.float32, device=dev))
+            g.append(torch.zeros(shapes[k % 2], dtype=F32, device=dev))
         else:
-            g.append(t.to(torch.float32).contiguous())
-    with torch.cuda.device(dev):
-        V = N * P1 + N * P2
-        gp = torch.empty((V, 3), dtype=torch.float32, device=dev) if need_points else None
-        gn = torch.empty((V, 3), dtype=torch.float32, device=dev) if need_normals else None
-        ws, ws_bytes = _chamfer_workspace(lib, N, P1, P2, 1, dev)
-        _lib.check(lib.b200r_chamfer_backward(
-            _ptr(x), _ptr(y), N, P1, P2, _ptr(xl), _ptr(yl), _ptr(xn), _ptr(yn), _ptr(w), int(norm), pr, br,
-            int(bool(single_directional)), int(bool(abs_cosine)), _ptr(idx_x), _ptr(idx_y), _ptr(cloud),
-            _ptr(argmax), _ptr(g[0]), _ptr(g[1]), _ptr(g[2]), _ptr(g[3]), ws.data_ptr(), ws_bytes, _ptr(gp),
-            _ptr(gn), _stream_ptr(dev)))
+            g.append(t.to(F32).contiguous())
+            named.append((name, g[-1], F32, shapes[k % 2]))
+    _require_cuda(("x", x), *[n[:2] for n in named])
+    for name, t, dtype, shape in named:
+        _check_tensor(name, t, dtype, shape, None, op)
+    x, y, xl, yl, xn, yn, w = (_c(t) for t in (x, y, x_lengths, y_lengths, x_normals, y_normals, weights))
+    V = N * P1 + N * P2
+    gp, gn = _outputs(dev, (need_points, (V, 3)), (need_normals, (V, 3)))
+    ws, ws_bytes = _workspace(dev, "chamfer", N, P1, P2, 1, required=True)
+    _launch(dev, "chamfer_backward", _ptr(x), _ptr(y), N, P1, P2, _ptr(xl), _ptr(yl), _ptr(xn), _ptr(yn), _ptr(w),
+            int(norm), pr, br, int(bool(single_directional)), int(bool(abs_cosine)), _ptr(idx_x), _ptr(idx_y),
+            _ptr(cloud), _ptr(argmax), _ptr(g[0]), _ptr(g[1]), _ptr(g[2]), _ptr(g[3]), _ptr(ws), ws_bytes, _ptr(gp),
+            _ptr(gn))
     gx, gy = (gp[:N * P1].view(N, P1, 3), gp[N * P1:].view(N, P2, 3)) if gp is not None else (None, None)
     gnx, gny = (gn[:N * P1].view(N, P1, 3), gn[N * P1:].view(N, P2, 3)) if gn is not None else (None, None)
     return gx, gy, gnx, gny
@@ -1462,102 +1315,87 @@ def _chamfer_nn(x, y, x_lengths=None, y_lengths=None, norm: int = 2):
 LAPLACIAN_METHODS = {"uniform": 0, "cot": 1, "cotcurv": 2}  # B200R_LAPLACIAN_*
 
 
-def _check_regularizer_inputs(op, verts, faces, mesh_first_vert, mesh_num_verts):
-    """(V, F, N, device) of float32 verts (V, 3), int64 faces (F, 3) and the int64 (N,) per-mesh vertex ranges, all on
-    one CUDA device, N >= 1; raises RuntimeError otherwise and for sizes past the kernels' limits (V < 2^31 - 1,
-    6F < 2^31)."""
-    dev = _require_cuda(("verts", verts), ("faces", faces), ("mesh_first_vert", mesh_first_vert),
-                        ("mesh_num_verts", mesh_num_verts))
-    if verts.dtype != torch.float32:
-        raise RuntimeError("%s: expected scalar type Float for verts but found %s" % (op, verts.dtype))
-    if faces.dtype != torch.int64:
-        raise RuntimeError("%s: expected scalar type Long for faces but found %s" % (op, faces.dtype))
-    if verts.dim() != 2 or verts.shape[1] != 3:
-        raise RuntimeError("%s: verts must be (V, 3), got %s" % (op, tuple(verts.shape)))
-    if faces.dim() != 2 or faces.shape[1] != 3:
-        raise RuntimeError("%s: faces must be (F, 3), got %s" % (op, tuple(faces.shape)))
-    N = int(mesh_first_vert.shape[0]) if mesh_first_vert.dim() == 1 else -1
-    for name, t in (("mesh_first_vert", mesh_first_vert), ("mesh_num_verts", mesh_num_verts)):
-        if t.dtype != torch.int64 or t.dim() != 1 or t.shape[0] != N or N < 1:
-            raise RuntimeError("%s: %s must be an int64 (N,) tensor with N >= 1 like mesh_first_vert, got %s %s"
-                               % (op, name, t.dtype, tuple(t.shape)))
-    V, F = int(verts.shape[0]), int(faces.shape[0])
-    if V >= (1 << 31) - 1 or 6 * F >= (1 << 31) or N >= (1 << 31):
-        raise RuntimeError("%s: at most 2^31 - 2 vertices and (2^31 - 1) / 6 faces, got V = %d, F = %d" % (op, V, F))
+def regularizer_sizes_ok(V: int, F: int, N: int):
+    """Whether the regulariser kernels take these sizes (b200r_regularizers_workspace_bytes)."""
+    return V < (1 << 31) - 1 and 6 * F < (1 << 31) and 1 <= N < (1 << 31)
+
+
+def _check_regularizer_inputs(op, verts, faces, mesh_first_vert, mesh_num_verts, *named):
+    """(V, F, N, device) of verts / faces and the int64 (N,) per-mesh vertex ranges on one CUDA device with the (name,
+    tensor) pairs `named`, within the kernels' size limits."""
+    V, F, dev = _check_verts_faces(op, verts, faces, ("mesh_first_vert", mesh_first_vert),
+                                   ("mesh_num_verts", mesh_num_verts), *named)
+    N = _check_ranges(op, "mesh_first_vert", mesh_first_vert, "mesh_num_verts", mesh_num_verts)
+    if not regularizer_sizes_ok(V, F, N):
+        raise RuntimeError("%s: at most 2^31 - 2 vertices, (2^31 - 1) / 6 faces and 1 to 2^31 - 1 meshes, got V = %d, "
+                           "F = %d, N = %d" % (op, V, F, N))
     return V, F, N, dev
 
 
-def _regularizer_workspace(lib, V, F, N, dev):
-    ws_bytes = int(lib.b200r_regularizers_workspace_bytes(V, F, N))
-    return torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None, ws_bytes
-
-
-def _check_workspace(workspace, ws_bytes, dev):
-    if workspace is None and ws_bytes == 0:
-        return
-    if (workspace is None or not workspace.is_cuda or workspace.device != dev or workspace.dtype != torch.uint8
+def _check_regularizer_workspace(workspace, V, F, N, dev):
+    """The bytes of the forward's workspace, which a backward hands back: uint8, contiguous, on dev, large enough."""
+    ws_bytes = _workspace_size("regularizers", V, F, N)
+    if not (workspace is None and ws_bytes == 0) and (
+            workspace is None or not workspace.is_cuda or workspace.device != dev or workspace.dtype != torch.uint8
             or workspace.numel() < ws_bytes or not workspace.is_contiguous()):
         raise RuntimeError("workspace must be the uint8 workspace of the matching forward on %s" % dev)
-
-
-def _check_grad_loss(grad_loss, dev):
-    g = _check_grad("grad_loss", grad_loss.reshape(()) if grad_loss.numel() == 1 else grad_loss, (), dev)
-    return g
+    return ws_bytes
 
 
 def mesh_edge_table(faces: torch.Tensor, V: int, mesh_first_vert: torch.Tensor, mesh_num_verts: torch.Tensor):
     """The edge table of the regularisers, for tests: faces (F,3) i64 with vertices in [0, V), the per-mesh vertex
     ranges -> (edges (E,2) i64, face_to_edge (F,3) i64, num_edges_per_mesh (N,) i64), PyTorch3D's edges_packed(),
     faces_packed_to_edges_packed() and num_edges_per_mesh().  Reads E on the host."""
-    verts = torch.empty((int(V), 3), dtype=torch.float32, device=faces.device) if faces.is_cuda else \
-        torch.empty((int(V), 3))
+    verts = torch.empty((int(V), 3), dtype=F32, device=faces.device) if faces.is_cuda else torch.empty((int(V), 3))
     V, F, N, dev = _check_regularizer_inputs("mesh_edge_table", verts, faces, mesh_first_vert, mesh_num_verts)
-    lib = _lib.load()
     f, first, num = faces.contiguous(), mesh_first_vert.contiguous(), mesh_num_verts.contiguous()
-    with torch.cuda.device(dev):
-        edges = torch.empty((3 * F, 2), dtype=torch.int64, device=dev)
-        face_to_edge = torch.empty((F, 3), dtype=torch.int64, device=dev)
-        counts = torch.empty((N,), dtype=torch.int64, device=dev)
-        E = torch.empty((1,), dtype=torch.int64, device=dev)
-        ws, ws_bytes = _regularizer_workspace(lib, V, F, N, dev)
-        _lib.check(lib.b200r_mesh_edge_table(_ptr(f), V, F, _ptr(first), _ptr(num), N, _ptr(ws), ws_bytes,
-                                             _ptr(edges), _ptr(face_to_edge), _ptr(counts), _ptr(E),
-                                             _stream_ptr(dev)))
+    edges = torch.empty((3 * F, 2), dtype=I64, device=dev)
+    face_to_edge = torch.empty((F, 3), dtype=I64, device=dev)
+    counts = torch.empty((N,), dtype=I64, device=dev)
+    E = torch.empty((1,), dtype=I64, device=dev)
+    ws, ws_bytes = _workspace(dev, "regularizers", V, F, N)
+    _launch(dev, "mesh_edge_table", _ptr(f), V, F, _ptr(first), _ptr(num), N, _ptr(ws), ws_bytes, _ptr(edges),
+            _ptr(face_to_edge), _ptr(counts), _ptr(E))
     return edges[:int(E.item())], face_to_edge, counts
+
+
+def _regularizer_forward(name, verts, faces, mesh_first_vert, mesh_num_verts, *params):
+    """(loss () f32, workspace) of the fused regulariser b200r_<name>."""
+    V, F, N, dev = _check_regularizer_inputs(name, verts, faces, mesh_first_vert, mesh_num_verts)
+    v, f, first, num = (t.contiguous() for t in (verts, faces, mesh_first_vert, mesh_num_verts))
+    loss = torch.empty((), dtype=F32, device=dev)
+    ws, ws_bytes = _workspace(dev, "regularizers", V, F, N)
+    _launch(dev, name, _ptr(v), V, _ptr(f), F, _ptr(first), _ptr(num), N, *params, _ptr(ws), ws_bytes,
+            loss.data_ptr())
+    return loss, ws
+
+
+def _regularizer_backward(name, grad_loss, verts, faces, mesh_first_vert, mesh_num_verts, workspace, *params):
+    """grad_verts (V,3) f32 of the fused regulariser b200r_<name>, from the forward's workspace."""
+    V, F, N, dev = _check_regularizer_inputs(name, verts, faces, mesh_first_vert, mesh_num_verts,
+                                             ("grad_loss", grad_loss))
+    _check_tensor("grad_loss", grad_loss.reshape(()) if grad_loss.numel() == 1 else grad_loss, F32, (), None, name)
+    ws_bytes = _check_regularizer_workspace(workspace, V, F, N, dev)
+    g, v, f, first, num = (t.contiguous() for t in (grad_loss, verts, faces, mesh_first_vert, mesh_num_verts))
+    grad_verts = torch.empty((V, 3), dtype=F32, device=dev)
+    _launch(dev, name, g.data_ptr(), _ptr(v), V, _ptr(f), F, _ptr(first), _ptr(num), N, *params, _ptr(workspace),
+            ws_bytes, _ptr(grad_verts))
+    return grad_verts
 
 
 def mesh_edge_loss_forward(verts, faces, mesh_first_vert, mesh_num_verts, target_length: float):
     """Fused pytorch3d.loss.mesh_edge_loss (DESIGN.md section 18) -> (loss () f32, workspace): the workspace holds the
     tables `mesh_edge_loss_backward` reads."""
-    V, F, N, dev = _check_regularizer_inputs("mesh_edge_loss_forward", verts, faces, mesh_first_vert, mesh_num_verts)
-    lib = _lib.load()
-    v, f = verts.contiguous(), faces.contiguous()
-    with torch.cuda.device(dev):
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        ws, ws_bytes = _regularizer_workspace(lib, V, F, N, dev)
-        _lib.check(lib.b200r_mesh_edge_loss_forward(_ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()),
-                                                    _ptr(mesh_num_verts.contiguous()), N, float(target_length),
-                                                    _ptr(ws), ws_bytes, loss.data_ptr(), _stream_ptr(dev)))
-    return loss, ws
+    return _regularizer_forward("mesh_edge_loss_forward", verts, faces, mesh_first_vert, mesh_num_verts,
+                                float(target_length))
 
 
 def mesh_edge_loss_backward(grad_loss, verts, faces, mesh_first_vert, mesh_num_verts, target_length: float,
                             workspace):
     """Backward of `mesh_edge_loss_forward` -> grad_verts (V,3) f32, from the forward's workspace (no sort).
     Deterministic, no atomics; grad_loss stays on the device."""
-    V, F, N, dev = _check_regularizer_inputs("mesh_edge_loss_backward", verts, faces, mesh_first_vert, mesh_num_verts)
-    g = _check_grad_loss(grad_loss, dev)
-    lib = _lib.load()
-    ws_bytes = int(lib.b200r_regularizers_workspace_bytes(V, F, N))
-    _check_workspace(workspace, ws_bytes, dev)
-    v, f = verts.contiguous(), faces.contiguous()
-    with torch.cuda.device(dev):
-        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
-        _lib.check(lib.b200r_mesh_edge_loss_backward(g.data_ptr(), _ptr(v), V, _ptr(f), F,
-                                                     _ptr(mesh_first_vert.contiguous()),
-                                                     _ptr(mesh_num_verts.contiguous()), N, float(target_length),
-                                                     _ptr(workspace), ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
-    return grad_verts
+    return _regularizer_backward("mesh_edge_loss_backward", grad_loss, verts, faces, mesh_first_vert, mesh_num_verts,
+                                 workspace, float(target_length))
 
 
 def _laplacian_method(method):
@@ -1570,17 +1408,7 @@ def mesh_laplacian_smoothing_forward(verts, faces, mesh_first_vert, mesh_num_ver
     """Fused pytorch3d.loss.mesh_laplacian_smoothing for method "uniform", "cot" or "cotcurv" (DESIGN.md section 18)
     -> (loss () f32, workspace)."""
     m = _laplacian_method(method)
-    V, F, N, dev = _check_regularizer_inputs("mesh_laplacian_smoothing_forward", verts, faces, mesh_first_vert,
-                                             mesh_num_verts)
-    lib = _lib.load()
-    v, f = verts.contiguous(), faces.contiguous()
-    with torch.cuda.device(dev):
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        ws, ws_bytes = _regularizer_workspace(lib, V, F, N, dev)
-        _lib.check(lib.b200r_mesh_laplacian_smoothing_forward(
-            _ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()), _ptr(mesh_num_verts.contiguous()), N, m,
-            _ptr(ws), ws_bytes, loss.data_ptr(), _stream_ptr(dev)))
-    return loss, ws
+    return _regularizer_forward("mesh_laplacian_smoothing_forward", verts, faces, mesh_first_vert, mesh_num_verts, m)
 
 
 def mesh_laplacian_smoothing_backward(grad_loss, verts, faces, mesh_first_vert, mesh_num_verts, method: str,
@@ -1588,53 +1416,21 @@ def mesh_laplacian_smoothing_backward(grad_loss, verts, faces, mesh_first_vert, 
     """Backward of `mesh_laplacian_smoothing_forward` -> grad_verts (V,3) f32, with L and its weights constant (no
     sort).  Deterministic, no atomics."""
     m = _laplacian_method(method)
-    V, F, N, dev = _check_regularizer_inputs("mesh_laplacian_smoothing_backward", verts, faces, mesh_first_vert,
-                                             mesh_num_verts)
-    g = _check_grad_loss(grad_loss, dev)
-    lib = _lib.load()
-    ws_bytes = int(lib.b200r_regularizers_workspace_bytes(V, F, N))
-    _check_workspace(workspace, ws_bytes, dev)
-    v, f = verts.contiguous(), faces.contiguous()
-    with torch.cuda.device(dev):
-        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
-        _lib.check(lib.b200r_mesh_laplacian_smoothing_backward(
-            g.data_ptr(), _ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()),
-            _ptr(mesh_num_verts.contiguous()), N, m, _ptr(workspace), ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
-    return grad_verts
+    return _regularizer_backward("mesh_laplacian_smoothing_backward", grad_loss, verts, faces, mesh_first_vert,
+                                 mesh_num_verts, workspace, m)
 
 
 def mesh_normal_consistency_forward(verts, faces, mesh_first_vert, mesh_num_verts):
     """Fused pytorch3d.loss.mesh_normal_consistency (DESIGN.md section 18) -> (loss () f32, workspace).  The face pairs
     are enumerated on the device: nothing reads the edge counts on the host."""
-    V, F, N, dev = _check_regularizer_inputs("mesh_normal_consistency_forward", verts, faces, mesh_first_vert,
-                                             mesh_num_verts)
-    lib = _lib.load()
-    v, f = verts.contiguous(), faces.contiguous()
-    with torch.cuda.device(dev):
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        ws, ws_bytes = _regularizer_workspace(lib, V, F, N, dev)
-        _lib.check(lib.b200r_mesh_normal_consistency_forward(
-            _ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()), _ptr(mesh_num_verts.contiguous()), N,
-            _ptr(ws), ws_bytes, loss.data_ptr(), _stream_ptr(dev)))
-    return loss, ws
+    return _regularizer_forward("mesh_normal_consistency_forward", verts, faces, mesh_first_vert, mesh_num_verts)
 
 
 def mesh_normal_consistency_backward(grad_loss, verts, faces, mesh_first_vert, mesh_num_verts, workspace):
     """Backward of `mesh_normal_consistency_forward` -> grad_verts (V,3) f32 (no sort, no scatter).  Deterministic,
     no atomics."""
-    V, F, N, dev = _check_regularizer_inputs("mesh_normal_consistency_backward", verts, faces, mesh_first_vert,
-                                             mesh_num_verts)
-    g = _check_grad_loss(grad_loss, dev)
-    lib = _lib.load()
-    ws_bytes = int(lib.b200r_regularizers_workspace_bytes(V, F, N))
-    _check_workspace(workspace, ws_bytes, dev)
-    v, f = verts.contiguous(), faces.contiguous()
-    with torch.cuda.device(dev):
-        grad_verts = torch.empty((V, 3), dtype=torch.float32, device=dev)
-        _lib.check(lib.b200r_mesh_normal_consistency_backward(
-            g.data_ptr(), _ptr(v), V, _ptr(f), F, _ptr(mesh_first_vert.contiguous()),
-            _ptr(mesh_num_verts.contiguous()), N, _ptr(workspace), ws_bytes, _ptr(grad_verts), _stream_ptr(dev)))
-    return grad_verts
+    return _regularizer_backward("mesh_normal_consistency_backward", grad_loss, verts, faces, mesh_first_vert,
+                                 mesh_num_verts, workspace)
 
 
 # the name the test hook is known by
@@ -1655,10 +1451,10 @@ def _clip_frustum_args(frustum):
     return planes, mask, int(z is not None), 0.0 if z is None else float(z), int(bool(frustum.perspective_correct))
 
 
-def _check_face_verts(face_verts):
-    if face_verts.dtype != torch.float32 or face_verts.dim() != 3 or tuple(face_verts.shape[1:]) != (3, 3):
-        raise RuntimeError("face_verts must be a float32 tensor of shape (F, 3, 3), got %s %s"
-                           % (face_verts.dtype, tuple(face_verts.shape)))
+def _check_clip_workspace(workspace, F):
+    """The int64 workspace of `clip_faces_count` for F faces."""
+    words = int(_lib.load().b200r_clip_faces_workspace_words(F))
+    _check_tensor("workspace", workspace, I64, (words,), "workspace words of clip_faces_count,")
 
 
 def clip_faces_count(frustum, face_verts=None, verts=None, faces=None):
@@ -1666,118 +1462,103 @@ def clip_faces_count(frustum, face_verts=None, verts=None, faces=None):
     verts[faces], read in place -- against `frustum` and returns the int64 workspace whose first four words are the
     record (F_clipped, n_case3, n_case4, number of faces culled or clipped).  Asynchronous: the caller reads the record."""
     if face_verts is not None:
-        _check_face_verts(face_verts)
         dev = _require_cuda(("face_verts", face_verts))
+        _check_tensor("face_verts", face_verts, F32, (None, 3, 3), "F, 3, 3")
         F = int(face_verts.shape[0])
         fv, v, f = face_verts.contiguous(), None, None
     else:
-        if verts.dtype != torch.float32 or verts.dim() != 2 or verts.shape[1] != 3:
-            raise RuntimeError("verts must be a float32 tensor of shape (V, 3), got %s %s"
-                               % (verts.dtype, tuple(verts.shape)))
-        if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
-            raise RuntimeError("faces must be an int64 tensor of shape (F, 3), got %s %s"
-                               % (faces.dtype, tuple(faces.shape)))
-        dev = _require_cuda(("verts", verts), ("faces", faces))
-        F = int(faces.shape[0])
+        _, F, dev = _check_verts_faces(None, verts, faces)
         fv, v, f = None, verts.contiguous(), faces.contiguous()
-    lib = _lib.load()
     planes, mask, has_z, z, _ = _clip_frustum_args(frustum)
-    with torch.cuda.device(dev):
-        ws = torch.empty((int(lib.b200r_clip_faces_workspace_words(F)),), dtype=torch.int64, device=dev)
-        _lib.check(lib.b200r_clip_faces_count(_ptr(fv), _ptr(v), _ptr(f), F, planes, mask, has_z, z, _ptr(ws),
-                                              _stream_ptr(dev)))
+    ws = torch.empty((int(_lib.load().b200r_clip_faces_workspace_words(F)),), dtype=I64, device=dev)
+    _launch(dev, "clip_faces_count", _ptr(fv), _ptr(v), _ptr(f), F, planes, mask, has_z, z, _ptr(ws))
     return ws
-
-
-def _check_clip_ranges(face_verts, mesh_to_face_first_idx, num_faces_per_mesh):
-    for name, t in (("mesh_to_face_first_idx", mesh_to_face_first_idx), ("num_faces_per_mesh", num_faces_per_mesh)):
-        if t.dtype != torch.int64 or t.dim() != 1:
-            raise RuntimeError("%s must be an int64 tensor of shape (N,), got %s %s" % (name, t.dtype, tuple(t.shape)))
-    if num_faces_per_mesh.shape[0] != mesh_to_face_first_idx.shape[0]:
-        raise RuntimeError("num_faces_per_mesh must have the same size as mesh_to_face_first_idx")
-    return _require_cuda(("face_verts", face_verts), ("mesh_to_face_first_idx", mesh_to_face_first_idx),
-                         ("num_faces_per_mesh", num_faces_per_mesh))
 
 
 def clip_faces_fill(face_verts, mesh_to_face_first_idx, num_faces_per_mesh, frustum, workspace, record):
     """Fill pass of the fused clip_faces: the seven ClippedFaces fields in the reference's layout, from the workspace of
     `clip_faces_count(frustum, face_verts)` and its record (a 4-sequence read by the caller).  The last three are empty
     tensors when no face was clipped (only culled)."""
-    _check_face_verts(face_verts)
-    dev = _check_clip_ranges(face_verts, mesh_to_face_first_idx, num_faces_per_mesh)
-    lib = _lib.load()
-    F, N = int(face_verts.shape[0]), int(mesh_to_face_first_idx.shape[0])
+    dev = _require_cuda(("face_verts", face_verts), ("mesh_to_face_first_idx", mesh_to_face_first_idx),
+                        ("num_faces_per_mesh", num_faces_per_mesh), ("workspace", workspace))
+    _check_tensor("face_verts", face_verts, F32, (None, 3, 3), "F, 3, 3")
+    F = int(face_verts.shape[0])
+    N = _check_ranges(None, "mesh_to_face_first_idx", mesh_to_face_first_idx, "num_faces_per_mesh", num_faces_per_mesh)
+    _check_clip_workspace(workspace, F)
     F_clipped, n3, n4 = (int(v) for v in record[:3])
     T = n3 + 2 * n4
     planes, mask, has_z, z, persp = _clip_frustum_args(frustum)
     fv, first = face_verts.contiguous(), mesh_to_face_first_idx.contiguous()
-    with torch.cuda.device(dev):
-        out_fv = torch.empty((F_clipped, 3, 3), dtype=torch.float32, device=dev)
-        out_first = torch.empty((N,), dtype=torch.int64, device=dev)
-        out_num = torch.empty((N,), dtype=torch.int64, device=dev)
-        c2u = torch.empty((F_clipped,), dtype=torch.int64, device=dev)
-        conv = torch.empty((T, 3, 3), dtype=torch.float32, device=dev)
-        conv_idx = torch.empty((F_clipped if T > 0 else 0,), dtype=torch.int64, device=dev)
-        neighbor = torch.empty((F_clipped if T > 0 else 0,), dtype=torch.int64, device=dev)
-        _lib.check(lib.b200r_clip_faces_fill(
-            _ptr(fv), F, _ptr(first), N, planes, mask, has_z, z, persp, _ptr(workspace), F_clipped, n3, n4,
-            _ptr(out_fv), _ptr(out_first), _ptr(out_num), _ptr(c2u), _ptr(conv), _ptr(conv_idx), _ptr(neighbor),
-            _stream_ptr(dev)))
+    out_fv = torch.empty((F_clipped, 3, 3), dtype=F32, device=dev)
+    out_first = torch.empty((N,), dtype=I64, device=dev)
+    out_num = torch.empty((N,), dtype=I64, device=dev)
+    c2u = torch.empty((F_clipped,), dtype=I64, device=dev)
+    conv = torch.empty((T, 3, 3), dtype=F32, device=dev)
+    conv_idx = torch.empty((F_clipped if T > 0 else 0,), dtype=I64, device=dev)
+    neighbor = torch.empty((F_clipped if T > 0 else 0,), dtype=I64, device=dev)
+    _launch(dev, "clip_faces_fill", _ptr(fv), F, _ptr(first), N, planes, mask, has_z, z, persp, _ptr(workspace),
+            F_clipped, n3, n4, _ptr(out_fv), _ptr(out_first), _ptr(out_num), _ptr(c2u), _ptr(conv), _ptr(conv_idx),
+            _ptr(neighbor))
     return out_fv, out_first, out_num, c2u, conv, conv_idx, neighbor
 
 
 def clip_faces_backward(face_verts, frustum, workspace, record, grad_face_verts_clipped, grad_conversion):
     """d loss / d face_verts (F,3,3) of the fused clip_faces from the gradients of its clipped face_verts and of its
     barycentric_conversion (either may be None); deterministic, no host synchronisation."""
-    _check_face_verts(face_verts)
-    dev = _require_cuda(("face_verts", face_verts), ("workspace", workspace))
-    n3, n4 = int(record[1]), int(record[2])
-    for name, g in (("grad_face_verts_clipped", grad_face_verts_clipped), ("grad_conversion", grad_conversion)):
-        if g is not None:
-            _require_cuda(("face_verts", face_verts), (name, g))
-            if g.dtype != torch.float32:
-                raise RuntimeError("%s must be float32, got %s" % (name, g.dtype))
-    lib = _lib.load()
+    grads = [(name, g, shape) for name, g, shape in (
+        ("grad_face_verts_clipped", grad_face_verts_clipped, (int(record[0]), 3, 3)),
+        ("grad_conversion", grad_conversion, (int(record[1]) + 2 * int(record[2]), 3, 3))) if g is not None]
+    dev = _require_cuda(("face_verts", face_verts), ("workspace", workspace), *[g[:2] for g in grads])
+    _check_tensor("face_verts", face_verts, F32, (None, 3, 3), "F, 3, 3")
     F = int(face_verts.shape[0])
+    _check_clip_workspace(workspace, F)
+    for name, g, shape in grads:
+        _check_tensor(name, g, F32, shape)
+    n3, n4 = int(record[1]), int(record[2])
     planes, mask, has_z, z, persp = _clip_frustum_args(frustum)
-    fv = face_verts.contiguous()
-    gfv = grad_face_verts_clipped.contiguous() if grad_face_verts_clipped is not None else None
-    gc = grad_conversion.contiguous() if grad_conversion is not None else None
-    with torch.cuda.device(dev):
-        grad = torch.empty((F, 3, 3), dtype=torch.float32, device=dev)
-        _lib.check(lib.b200r_clip_faces_backward(_ptr(fv), F, planes, mask, has_z, z, persp, _ptr(workspace), n3, n4,
-                                                 _ptr(gfv), _ptr(gc), _ptr(grad), _stream_ptr(dev)))
+    fv, gfv, gc = (_c(t) for t in (face_verts, grad_face_verts_clipped, grad_conversion))
+    grad = torch.empty((F, 3, 3), dtype=F32, device=dev)
+    _launch(dev, "clip_faces_backward", _ptr(fv), F, planes, mask, has_z, z, persp, _ptr(workspace), n3, n4, _ptr(gfv),
+            _ptr(gc), _ptr(grad))
     return grad
+
+
+def _check_clip_convert_inputs(pix_to_face, barycentric_coords, conversion, grad=None):
+    """The device of pix_to_face (any shape) i64 with its float32 barycentric_coords (pix_to_face.shape + (3,)), of the
+    (name, tensor) clipped-face maps `conversion` -- int64 (F_clipped,) indices and the float32 (T, 3, 3)
+    barycentric_conversion -- and of the float32 upstream gradient (name, tensor) of barycentric_coords when given."""
+    dev = _require_cuda(*([grad] if grad is not None else []), ("pix_to_face", pix_to_face),
+                        ("barycentric_coords", barycentric_coords), *conversion)
+    _check_tensor("pix_to_face", pix_to_face, I64)
+    bary_shape = tuple(pix_to_face.shape) + (3,)
+    _check_tensor("barycentric_coords", barycentric_coords, F32, bary_shape, "pix_to_face.shape + (3,)")
+    for name, t in conversion:
+        if name == "barycentric_conversion":
+            _check_tensor(name, t, F32, (None, 3, 3), "T, 3, 3")
+        else:
+            _check_tensor(name, t, I64, (None,), "F_clipped,")
+    if grad is not None:
+        _check_tensor(*grad, F32, bary_shape, "pix_to_face.shape + (3,)")
+    return dev
 
 
 def clip_convert_forward(pix_to_face, barycentric_coords, faces_clipped_to_unclipped_idx, barycentric_conversion=None,
                          faces_clipped_to_conversion_idx=None):
     """Fused convert_clipped_rasterization_to_original_faces: (pix_to_face_unclipped, bary_unclipped).  Without a
     conversion only pix_to_face is mapped and bary_unclipped is None."""
-    if pix_to_face.dtype != torch.int64:
-        raise RuntimeError("pix_to_face must be int64, got %s" % pix_to_face.dtype)
-    if barycentric_coords.dtype != torch.float32 or tuple(barycentric_coords.shape) != tuple(pix_to_face.shape) + (3,):
-        raise RuntimeError("barycentric_coords must be a float32 tensor of shape pix_to_face.shape + (3,), got %s %s"
-                           % (barycentric_coords.dtype, tuple(barycentric_coords.shape)))
-    named = [("pix_to_face", pix_to_face), ("barycentric_coords", barycentric_coords),
-             ("faces_clipped_to_unclipped_idx", faces_clipped_to_unclipped_idx)]
+    conversion = [("faces_clipped_to_unclipped_idx", faces_clipped_to_unclipped_idx)]
     if barycentric_conversion is not None:
-        if barycentric_conversion.dtype != torch.float32 or tuple(barycentric_conversion.shape[1:]) != (3, 3):
-            raise RuntimeError("barycentric_conversion must be a float32 tensor of shape (T, 3, 3), got %s %s"
-                               % (barycentric_conversion.dtype, tuple(barycentric_conversion.shape)))
-        named += [("barycentric_conversion", barycentric_conversion),
-                  ("faces_clipped_to_conversion_idx", faces_clipped_to_conversion_idx)]
-    dev = _require_cuda(*named)
-    lib = _lib.load()
+        conversion += [("barycentric_conversion", barycentric_conversion),
+                       ("faces_clipped_to_conversion_idx", faces_clipped_to_conversion_idx)]
+    dev = _check_clip_convert_inputs(pix_to_face, barycentric_coords, conversion)
     p2f, bary = pix_to_face.contiguous(), barycentric_coords.contiguous()
     c2u = faces_clipped_to_unclipped_idx.contiguous()
     conv = barycentric_conversion.contiguous() if barycentric_conversion is not None else None
     cidx = faces_clipped_to_conversion_idx.contiguous() if barycentric_conversion is not None else None
-    with torch.cuda.device(dev):
-        p2f_out = torch.empty_like(p2f)
-        bary_out = torch.empty_like(bary) if conv is not None else None
-        _lib.check(lib.b200r_clip_convert_forward(_ptr(p2f), _ptr(bary), p2f.numel(), _ptr(c2u), _ptr(conv),
-                                                  _ptr(cidx), _ptr(p2f_out), _ptr(bary_out), _stream_ptr(dev)))
+    p2f_out = torch.empty_like(p2f)
+    bary_out = torch.empty_like(bary) if conv is not None else None
+    _launch(dev, "clip_convert_forward", _ptr(p2f), _ptr(bary), p2f.numel(), _ptr(c2u), _ptr(conv), _ptr(cidx),
+            _ptr(p2f_out), _ptr(bary_out))
     return p2f_out, bary_out
 
 
@@ -1786,28 +1567,20 @@ def clip_convert_backward(grad_bary_unclipped, pix_to_face, barycentric_coords, 
     """Backward of `clip_convert_forward` -> (grad_barycentric_coords, grad_conversion); an entry is None where
     `needs_input_grad` (same order) is false.  grad_conversion is accumulated with atomics, so requesting it under
     torch.use_deterministic_algorithms(True) raises, like the rasterizer backward in the same graph."""
-    dev = _require_cuda(("grad_bary_unclipped", grad_bary_unclipped), ("pix_to_face", pix_to_face),
-                        ("barycentric_coords", barycentric_coords), ("barycentric_conversion", barycentric_conversion),
-                        ("faces_clipped_to_conversion_idx", faces_clipped_to_conversion_idx))
-    if grad_bary_unclipped.dtype != torch.float32 or grad_bary_unclipped.shape != barycentric_coords.shape:
-        raise RuntimeError("grad_bary_unclipped must be a float32 tensor of shape %s, got %s %s"
-                           % (tuple(barycentric_coords.shape), grad_bary_unclipped.dtype,
-                              tuple(grad_bary_unclipped.shape)))
+    dev = _check_clip_convert_inputs(pix_to_face, barycentric_coords,
+                                     [("barycentric_conversion", barycentric_conversion),
+                                      ("faces_clipped_to_conversion_idx", faces_clipped_to_conversion_idx)],
+                                     ("grad_bary_unclipped", grad_bary_unclipped))
     need_bary, need_conv = (bool(v) for v in needs_input_grad)
-    if need_conv and torch.are_deterministic_algorithms_enabled() and \
-            not torch.is_deterministic_algorithms_warn_only_enabled():
-        raise RuntimeError(
-            "clip_convert_backward does not have a deterministic implementation (grad_conversion is accumulated with "
-            "atomics), but you set 'torch.use_deterministic_algorithms(True)'.")
-    lib = _lib.load()
+    if need_conv:
+        _refuse_nondeterministic("clip_convert_backward", "grad_conversion is accumulated with atomics")
     g, p2f, bary = grad_bary_unclipped.contiguous(), pix_to_face.contiguous(), barycentric_coords.contiguous()
     conv, cidx = barycentric_conversion.contiguous(), faces_clipped_to_conversion_idx.contiguous()
     T = int(conv.shape[0])
-    with torch.cuda.device(dev):
-        g_bary = torch.empty_like(bary) if need_bary else None
-        g_conv = torch.empty_like(conv) if need_conv else None
-        _lib.check(lib.b200r_clip_convert_backward(_ptr(g), _ptr(p2f), _ptr(bary), p2f.numel(), _ptr(conv), _ptr(cidx),
-                                                   T, _ptr(g_bary), _ptr(g_conv), _stream_ptr(dev)))
+    g_bary = torch.empty_like(bary) if need_bary else None
+    g_conv = torch.empty_like(conv) if need_conv else None
+    _launch(dev, "clip_convert_backward", _ptr(g), _ptr(p2f), _ptr(bary), p2f.numel(), _ptr(conv), _ptr(cidx), T,
+            _ptr(g_bary), _ptr(g_conv))
     return g_bary, g_conv
 
 
@@ -1815,42 +1588,42 @@ def clip_convert_backward(grad_bary_unclipped, pix_to_face, barycentric_coords, 
 # pytorch3d/csrc/ext.cpp:69-73: "These are only visible for testing; users should not call them directly".  Provided so
 # that the reference's own tests of these entry points can run against this build; none of them is on the product path.
 
-def _coarse(fn_name, elems, first, num, image_size, bin_size, max_per_bin, blur_radius=None, radius=None):
-    dev = _require_cuda(("elements", elems), ("first_idx", first), ("num_per_batch", num))
-    lib = _lib.load()
+def _coarse(kind, elems, first, num, image_size, bin_size, max_per_bin, blur_radius=None, radius=None):
+    dev = _require_cuda(("elements", elems), ("first_idx", first), ("num_per_batch", num),
+                        *([("radius", radius)] if radius is not None else []))
     H, W = int(image_size[0]), int(image_size[1])
     N, E = int(num.shape[0]), int(elems.shape[0])
+    el = elems.contiguous()
+    f64, n64 = first.contiguous().to(I64), num.contiguous().to(I64)
+    _check_tensor("elements", el, F32)
+    _check_tensor("num_per_batch", n64, I64, (N,), "N,")
+    _check_tensor("first_idx", f64, I64, (N,), "N,")
+    if radius is not None:
+        _check_tensor("radius", radius, F32, (E,), "num_points,")
     bin_size, M = int(bin_size), int(max_per_bin)
     if bin_size <= 0:
         raise RuntimeError("bin_size must be positive for the coarse stage")
     BH, BW = 1 + (H - 1) // bin_size, 1 + (W - 1) // bin_size
     if BH >= 22 or BW >= 22:  # kMaxItemsPerBin (rasterize_coarse.cu:244-249)
         raise RuntimeError("In RasterizeCoarseCuda got num_bins_y: %d, num_bins_x: %d, too many bins" % (BH, BW))
-    el = elems.contiguous()
-    f64, n64 = first.contiguous().to(torch.int64), num.contiguous().to(torch.int64)
-    with torch.cuda.device(dev):
-        bins = torch.empty((N, BH, BW, M), dtype=torch.int32, device=dev)
-        counts = torch.empty((N, BH, BW), dtype=torch.int32, device=dev)
-        overflow = torch.zeros((1,), dtype=torch.int32, device=dev)
-        if blur_radius is not None:
-            _lib.check(lib.b200r_rasterize_meshes_coarse(_ptr(el), E, _ptr(f64), _ptr(n64), N, H, W, float(blur_radius),
-                                                         bin_size, M, bins.data_ptr(), counts.data_ptr(),
-                                                         overflow.data_ptr(), _stream_ptr(dev)))
-        else:
-            rad = radius.contiguous()
-            _lib.check(lib.b200r_rasterize_points_coarse(_ptr(el), E, _ptr(f64), _ptr(n64), _ptr(rad), N, H, W, bin_size,
-                                                         M, bins.data_ptr(), counts.data_ptr(), overflow.data_ptr(),
-                                                         _stream_ptr(dev)))
-        if int(overflow.item()) != 0:
-            import warnings
-            warnings.warn("Bin size was too small in the coarse rasterization phase. This caused an overflow, meaning "
-                          "output may be incomplete. To solve, try increasing max_faces_per_bin / max_points_per_bin, "
-                          "decreasing bin_size, or setting bin_size to 0 to use the naive rasterization.")
-        # canonical form: ascending element index inside every bin, -1 padding last
-        big = torch.iinfo(torch.int32).max
-        bins = torch.where(bins < 0, torch.full_like(bins, big), bins).sort(dim=-1).values
-        bins = torch.where(bins == big, torch.full_like(bins, -1), bins)
-    return bins
+    bins = torch.empty((N, BH, BW, M), dtype=I32, device=dev)
+    counts = torch.empty((N, BH, BW), dtype=I32, device=dev)
+    overflow = torch.zeros((1,), dtype=I32, device=dev)
+    if blur_radius is not None:
+        args = (_ptr(el), E, _ptr(f64), _ptr(n64), N, H, W, float(blur_radius))
+    else:
+        args = (_ptr(el), E, _ptr(f64), _ptr(n64), _ptr(radius.contiguous()), N, H, W)
+    _launch(dev, "rasterize_%s_coarse" % kind, *args, bin_size, M, bins.data_ptr(), counts.data_ptr(),
+            overflow.data_ptr())
+    if int(overflow.item()) != 0:
+        import warnings
+        warnings.warn("Bin size was too small in the coarse rasterization phase. This caused an overflow, meaning "
+                      "output may be incomplete. To solve, try increasing max_faces_per_bin / max_points_per_bin, "
+                      "decreasing bin_size, or setting bin_size to 0 to use the naive rasterization.")
+    # canonical form: ascending element index inside every bin, -1 padding last
+    big = torch.iinfo(torch.int32).max
+    bins = torch.where(bins < 0, torch.full_like(bins, big), bins).sort(dim=-1).values
+    return torch.where(bins == big, torch.full_like(bins, -1), bins)
 
 
 def _rasterize_meshes_coarse(face_verts, mesh_to_face_first_idx, num_faces_per_mesh, image_size, blur_radius, bin_size,

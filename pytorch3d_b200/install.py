@@ -550,7 +550,7 @@ def _mesh_fused(verts, faces):
         return False
     if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
         return False
-    return verts.shape[0] < (1 << 31) - 1 and 3 * faces.shape[0] < (1 << 31)
+    return _b200_C.normals_sizes_ok(int(verts.shape[0]), int(faces.shape[0]))
 
 
 def _face_normals_fused(name, args):
@@ -598,11 +598,12 @@ def install_normals():
 
 def _regularizer_fused(meshes):
     """Whether the fused regularisers take this batch: at least one mesh, float32 CUDA verts and int64 CUDA faces on
-    one device, V < 2^31 - 1 and 6F < 2^31."""
+    one device, within the kernels' size limits."""
     if len(meshes) == 0:
         return False
     verts, faces = meshes.verts_packed(), meshes.faces_packed()
-    return _mesh_fused(verts, faces) and 6 * faces.shape[0] < (1 << 31)
+    return _mesh_fused(verts, faces) and _b200_C.regularizer_sizes_ok(int(verts.shape[0]), int(faces.shape[0]),
+                                                                      len(meshes))
 
 
 def _regularizer_dispatch(name, original):
