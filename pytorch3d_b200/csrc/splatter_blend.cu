@@ -122,17 +122,17 @@ __device__ __forceinline__ void stage_slots(float* sm, int kcs, const float* __r
 }
 
 // Forward (RECORD = false: writes out) and the backward's record kernel (RECORD = true: reads grad_out, writes the
-// record).  One thread per pixel of a 32 x 8 tile.
+// record).  One thread per pixel of a 32 x 8 tile; image n0 + blockIdx.z, tile row ty0 + blockIdx.y.
 template <bool RECORD>
 __global__ void __launch_bounds__(kSplatThreads)
     splatter_blend_pixel_kernel(const float* __restrict__ colors, const float* __restrict__ coords,
-                                const uint8_t* __restrict__ mask, int H, int W, int K, SplatArgs s,
+                                const uint8_t* __restrict__ mask, int n0, int ty0, int H, int W, int K, SplatArgs s,
                                 const float* __restrict__ grad_out, float* __restrict__ out) {
   extern __shared__ float sm[];
   const int kcs = K < kSplatChunk ? K : kSplatChunk;  // slots per staged chunk
   const int nchunk = (K + kSplatChunk - 1) / kSplatChunk;
-  const int64_t n = blockIdx.z;
-  const int y0 = blockIdx.y * kSplatTileH, x0 = blockIdx.x * kSplatTileW;
+  const int64_t n = n0 + blockIdx.z;  // unsigned: n >= 0 is known to the compiler
+  const int y0 = (ty0 + blockIdx.y) * kSplatTileH, x0 = blockIdx.x * kSplatTileW;
   const int tx = threadIdx.x % kSplatTileW, ty = threadIdx.x / kSplatTileW;
   const float norm = splat_norm(s.inv);
   const int self = (ty + 1) * kSplatHaloW + tx + 1;
@@ -279,12 +279,12 @@ __global__ void __launch_bounds__(kSplatThreads)
 // splats were dropped by the reference's padding).
 __global__ void __launch_bounds__(kSplatThreads)
     splatter_blend_gather_kernel(const float* __restrict__ colors, const float* __restrict__ coords,
-                                 const uint8_t* __restrict__ mask, int H, int W, int K, SplatArgs s,
+                                 const uint8_t* __restrict__ mask, int n0, int ty0, int H, int W, int K, SplatArgs s,
                                  const float* __restrict__ record, float* __restrict__ grad_colors,
                                  float* __restrict__ grad_coords) {
   __shared__ float rs[kRecordFields * kSplatHalo];
-  const int64_t n = blockIdx.z;
-  const int y0 = blockIdx.y * kSplatTileH, x0 = blockIdx.x * kSplatTileW;
+  const int64_t n = n0 + blockIdx.z;  // unsigned: n >= 0 is known to the compiler
+  const int y0 = (ty0 + blockIdx.y) * kSplatTileH, x0 = blockIdx.x * kSplatTileW;
   const float norm = splat_norm(s.inv);
   for (int i = threadIdx.x; i < kSplatHalo * kRecordFields; i += kSplatThreads) {
     const int pos = i / kRecordFields, f = i - pos * kRecordFields;
@@ -350,9 +350,20 @@ static int splatter_args(int32_t N, int32_t H, int32_t W, int32_t K, double sigm
   return B200R_OK;
 }
 
-static dim3 splatter_grid(int32_t N, int32_t H, int32_t W) {
-  return dim3((unsigned)((W + kSplatTileW - 1) / kSplatTileW), (unsigned)((H + kSplatTileH - 1) / kSplatTileH),
-              (unsigned)N);
+// Both kernels are launched over the images and tile rows in chunks of at most 65535, the limit of grid.y and grid.z;
+// each launch gets its first image n0 and first tile row ty0.  f(grid, n0, ty0) launches one chunk and returns its
+// status; the first failure stops the launches.
+template <typename Launch>
+static int for_each_splatter_chunk(int32_t N, int32_t H, int32_t W, Launch f) {
+  constexpr int kMaxGridYZ = 65535;
+  const int TX = (W + kSplatTileW - 1) / kSplatTileW, TY = (H + kSplatTileH - 1) / kSplatTileH;
+  for (int n0 = 0; n0 < N; n0 += kMaxGridYZ)
+    for (int ty0 = 0; ty0 < TY; ty0 += kMaxGridYZ) {
+      const int rc = f(dim3((unsigned)TX, (unsigned)min(TY - ty0, kMaxGridYZ), (unsigned)min(N - n0, kMaxGridYZ)),
+                       n0, ty0);
+      if (rc != B200R_OK) return rc;
+    }
+  return B200R_OK;
 }
 
 template <bool RECORD>
@@ -363,10 +374,12 @@ static int launch_pixel_kernel(const float* colors, const float* coords, const u
   const size_t smem = (size_t)kSplatFields * kcs * kSplatHalo * sizeof(float);  // 76,160 bytes at K >= 8
   B200R_CUDA_OK(cudaFuncSetAttribute(splatter_blend_pixel_kernel<RECORD>,
                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  splatter_blend_pixel_kernel<RECORD><<<splatter_grid(N, H, W), kSplatThreads, smem, stream>>>(
-      colors, coords, mask, H, W, K, s, grad_out, out);
-  B200R_LAUNCHED(RECORD ? "splatter_blend_pixel_kernel<record>" : "splatter_blend_pixel_kernel<forward>");
-  return B200R_OK;
+  return for_each_splatter_chunk(N, H, W, [&](dim3 grid, int n0, int ty0) {
+    splatter_blend_pixel_kernel<RECORD><<<grid, kSplatThreads, smem, stream>>>(colors, coords, mask, n0, ty0, H, W, K,
+                                                                               s, grad_out, out);
+    B200R_LAUNCHED(RECORD ? "splatter_blend_pixel_kernel<record>" : "splatter_blend_pixel_kernel<forward>");
+    return B200R_OK;
+  });
 }
 
 extern "C" int b200r_splatter_blend_forward(const float* colors, const float* pixel_coords_screen,
@@ -405,8 +418,11 @@ extern "C" int b200r_splatter_blend_backward(const float* grad_out, const float*
   float* record = static_cast<float*>(workspace);
   rc = launch_pixel_kernel<true>(colors, pixel_coords_screen, background_mask, N, H, W, K, s, grad_out, record, stream);
   if (rc != B200R_OK) return rc;
-  splatter_blend_gather_kernel<<<splatter_grid(N, H, W), kSplatThreads, 0, stream>>>(
-      colors, pixel_coords_screen, background_mask, H, W, K, s, record, grad_colors, grad_pixel_coords_screen);
-  B200R_LAUNCHED("splatter_blend_gather_kernel");
-  return B200R_OK;
+  return for_each_splatter_chunk(N, H, W, [&](dim3 grid, int n0, int ty0) {
+    splatter_blend_gather_kernel<<<grid, kSplatThreads, 0, stream>>>(colors, pixel_coords_screen, background_mask, n0,
+                                                                     ty0, H, W, K, s, record, grad_colors,
+                                                                     grad_pixel_coords_screen);
+    B200R_LAUNCHED("splatter_blend_gather_kernel");
+    return B200R_OK;
+  });
 }
