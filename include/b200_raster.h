@@ -786,6 +786,34 @@ int b200r_rasterize_points_coarse(const float* points, int64_t P, const int64_t*
                                   int32_t* bin_counts, int32_t* overflow, void* stream);
 
 /*
+ * Farthest point sampling and ball query (DESIGN.md section 22): pytorch3d.ops.sample_farthest_points and
+ * pytorch3d.ops.ball_query for D = 3, bit for bit what the reference's CUDA kernels compute.  Points are contiguous
+ * float32 (N, P, 3) device arrays, lengths int64 (N,) or NULL (all P), clamped to [0, P].  All entry points are
+ * asynchronous, use no float atomics and are deterministic.
+ *
+ * sample_farthest_points: idx (N, max_K) int64.  Row n is start_idxs[n], then min(K[n], lengths[n]) - 1 selections,
+ *  then -1; a start index outside [0, lengths[n]) of a non-empty cloud gives a row of -1.  K[n] > max_K is read as
+ *  max_K.  cluster_size 0 lets the library choose the CTAs per cloud (1 to 16), else forces it.  scratch: N P floats,
+ *  or NULL when the clouds fit on chip (the call fails otherwise).  P < 2^31.
+ * ball_query_forward: idx (N, P1, K) int64, dists (N, P1, K) float32 and, unless NULL, nn (N, P1, K, 3) float32: the
+ *  first K targets j in ascending order with dist2 < radius * radius (float32), padded with -1, 0 and 0.  With
+ *  skip_points_outside_cube and radius < 0 nothing is found.  N P1 K < 2^31 and N P2 < 2^31.
+ * ball_query_backward: grad_dists (N, P1, K) and grad_nn (N, P1, K, 3), either NULL -> grad_p1 (N, P1, 3) and
+ *  grad_p2 (N, P2, 3), either NULL.  workspace: b200r_ball_query_workspace_bytes(N, P1, P2, K) bytes.
+ */
+int b200r_sample_farthest_points(const float* points, int64_t N, int64_t P, const int64_t* lengths, const int64_t* K,
+                                 const int64_t* start_idxs, int64_t max_K, int32_t cluster_size, float* scratch,
+                                 int64_t* idx, void* stream);
+size_t b200r_ball_query_workspace_bytes(int64_t N, int64_t P1, int64_t P2, int64_t K);
+int b200r_ball_query_forward(const float* p1, const float* p2, int64_t N, int64_t P1, int64_t P2,
+                             const int64_t* lengths1, const int64_t* lengths2, int64_t K, float radius,
+                             int32_t skip_points_outside_cube, int64_t* idx, float* dists, float* nn, void* stream);
+int b200r_ball_query_backward(const float* p1, const float* p2, int64_t N, int64_t P1, int64_t P2,
+                              const int64_t* lengths1, const int64_t* lengths2, int64_t K, const int64_t* idx,
+                              const float* grad_dists, const float* grad_nn, void* workspace, size_t workspace_bytes,
+                              float* grad_p1, float* grad_p2, void* stream);
+
+/*
  * Programmatic dependent launch between the kernels of one call (setup -> scan -> fill -> fine; backward -> scatter):
  * the next kernel is made resident while its predecessor drains.  On by default; results never depend on it.
  */

@@ -1312,6 +1312,122 @@ def _chamfer_nn(x, y, x_lengths=None, y_lengths=None, norm: int = 2):
     return state[0], state[1].long(), state[2], state[3].long()
 
 
+# ------------------------------------------- farthest point sampling and ball query (DESIGN.md section 22)
+
+def fps_sizes_ok(P: int):
+    """Whether the farthest-point-sampling kernel takes clouds of P points: its keys hold the index in 32 bits."""
+    return 0 <= P < (1 << 31)
+
+
+def ball_query_sizes_ok(N: int, P1: int, P2: int, K: int):
+    """Whether the ball query kernels take these sizes: the backward's sort ids and keys are int32."""
+    return min(N, P1, P2, K) >= 0 and N * P1 * K < (1 << 31) and N * P2 < (1 << 31)
+
+
+def sample_farthest_points(points: torch.Tensor, lengths: torch.Tensor, K: torch.Tensor, start_idxs: torch.Tensor,
+                           max_K_known: int = -1, cluster_size: int = 0):
+    """pytorch3d._C.sample_farthest_points for D = 3: idx (N, max_K) int64 (DESIGN.md section 22).  max_K is
+    max_K_known when it is positive, else max(K), which synchronises the host once.  cluster_size 0 lets the library
+    choose the CTAs per cloud; 1 to 16 forces it (a test and timing hook)."""
+    op = "sample_farthest_points"
+    dev = _require_cuda(("points", points), ("lengths", lengths), ("K", K), ("start_idxs", start_idxs))
+    _check_tensor("points", points, F32, (None, None, 3), "N, P, 3", op)
+    N, P = int(points.shape[0]), int(points.shape[1])
+    if lengths.dim() != 1 or lengths.shape[0] != N:
+        raise RuntimeError("Point and lengths must have the same batch dimension")
+    if K.dim() != 1 or K.shape[0] != N:
+        raise RuntimeError("Points and K must have the same batch dimension")
+    for name, t in (("lengths", lengths), ("K", K), ("start_idxs", start_idxs)):
+        _check_tensor(name, t, I64, (N,), "N,", op)
+    if not fps_sizes_ok(P):
+        raise RuntimeError("%s: takes P < 2^31, got P = %d" % (op, P))
+    if not 0 <= int(cluster_size) <= 16:
+        raise RuntimeError("%s: cluster_size must be 0 to 16" % op)
+    max_K = int(max_K_known) if max_K_known > 0 else int(K.max())
+    idx = torch.empty((N, max_K), dtype=I64, device=dev)
+    if idx.numel() == 0:
+        return idx
+    if P == 0:  # FarthestPointSamplingCuda returns its -1 fill before any launch
+        return idx.fill_(-1)
+    points, lengths, K, start_idxs = (t.contiguous() for t in (points, lengths, K, start_idxs))
+    scratch = torch.empty((N, P), dtype=F32, device=dev)
+    _launch(dev, "sample_farthest_points", _ptr(points), N, P, _ptr(lengths), _ptr(K), _ptr(start_idxs), max_K,
+            int(cluster_size), _ptr(scratch), _ptr(idx))
+    return idx
+
+
+def _check_ball_inputs(op, p1, p2, lengths1, lengths2, *named):
+    """(N, P1, P2, device): float32 p1 (N, P1, 3) and p2 (N, P2, 3), int64 (N,) lengths (or None), and the (name,
+    tensor, dtype, shape) entries of `named` with None standing for N, P1, all on one CUDA device."""
+    dev = _require_cuda(*[(k, t) for k, t in (("p1", p1), ("p2", p2), ("lengths1", lengths1), ("lengths2", lengths2))
+                          if t is not None], *[(k, t) for k, t, _, _ in named if t is not None])
+    _check_tensor("p1", p1, F32, (None, None, 3), "N, P1, 3", op)
+    N, P1 = int(p1.shape[0]), int(p1.shape[1])
+    _check_tensor("p2", p2, F32, (N, None, 3), "N, P2, 3", op)
+    for name, t in (("lengths1", lengths1), ("lengths2", lengths2)):
+        if t is not None:
+            _check_tensor(name, t, I64, (N,), "N,", op)
+    for name, t, dtype, shape in named:
+        if t is not None:
+            _check_tensor(name, t, dtype, shape, None, op)
+    return N, P1, int(p2.shape[1]), dev
+
+
+def ball_query_forward(p1, p2, lengths1, lengths2, K: int, radius: float, skip_points_outside_cube: bool,
+                       return_nn: bool):
+    """Ball query for D = 3 (DESIGN.md section 22): (idx (N, P1, K) int64, dists (N, P1, K) float32, nn (N, P1, K, 3)
+    float32 or None), idx and dists bit for bit the reference's BallQueryCuda, nn what masked_gather(p2, idx) gives.
+    Lengths may be None (all P).  No host synchronisation."""
+    op = "ball_query_forward"
+    N, P1, P2, dev = _check_ball_inputs(op, p1, p2, lengths1, lengths2)
+    K = int(K)
+    if K < 0:
+        raise RuntimeError("Trying to create tensor with negative dimension %d: [%d, %d, %d]" % (K, N, P1, K))
+    if not ball_query_sizes_ok(N, P1, P2, K):
+        raise RuntimeError("%s: takes N P1 K < 2^31 and N P2 < 2^31, got N = %d, P1 = %d, P2 = %d, K = %d"
+                           % (op, N, P1, P2, K))
+    p1, p2, l1, l2 = (_c(t) for t in (p1, p2, lengths1, lengths2))
+    idx = torch.empty((N, P1, K), dtype=I64, device=dev)
+    dists = torch.empty((N, P1, K), dtype=F32, device=dev)
+    nn = torch.empty((N, P1, K, 3), dtype=F32, device=dev) if return_nn else None
+    if idx.numel() > 0:
+        _launch(dev, "ball_query_forward", _ptr(p1), _ptr(p2), N, P1, P2, _ptr(l1), _ptr(l2), K, float(radius),
+                int(bool(skip_points_outside_cube)), _ptr(idx), _ptr(dists), _ptr(nn))
+    return idx, dists, nn
+
+
+def ball_query(p1, p2, lengths1, lengths2, K: int, radius: float, skip_points_outside_cube: bool):
+    """pytorch3d._C.ball_query for D = 3: (idx, dists)."""
+    idx, dists, _ = ball_query_forward(p1, p2, lengths1, lengths2, K, radius, skip_points_outside_cube, False)
+    return idx, dists
+
+
+def ball_query_backward(p1, p2, lengths1, lengths2, idx, grad_dists, grad_nn, need_p1: bool = True,
+                        need_p2: bool = True):
+    """Backward of `ball_query_forward` -> (grad_p1 (N, P1, 3), grad_p2 (N, P2, 3)), each None unless asked for.
+    grad_dists (N, P1, K) and grad_nn (N, P1, K, 3) are the upstream gradients of dists and nn, either None.
+    Deterministic, no float atomics, no host synchronisation."""
+    op = "ball_query_backward"
+    _check_tensor("idx", idx, I64, (None, None, None), "N, P1, K", op)
+    N, P1, K = (int(v) for v in idx.shape)
+    grad_dists = grad_dists.to(F32).contiguous() if grad_dists is not None else None
+    grad_nn = grad_nn.to(F32).contiguous() if grad_nn is not None else None
+    N, P1, P2, dev = _check_ball_inputs(op, p1, p2, lengths1, lengths2, ("idx", idx, I64, (N, P1, K)),
+                                        ("grad_dists", grad_dists, F32, (N, P1, K)),
+                                        ("grad_nn", grad_nn, F32, (N, P1, K, 3)))
+    if not ball_query_sizes_ok(N, P1, P2, K):
+        raise RuntimeError("%s: takes N P1 K < 2^31 and N P2 < 2^31, got N = %d, P1 = %d, P2 = %d, K = %d"
+                           % (op, N, P1, P2, K))
+    gp1, gp2 = _outputs(dev, (need_p1, (N, P1, 3)), (need_p2, (N, P2, 3)))
+    if gp1 is None and gp2 is None:
+        return None, None
+    p1, p2, l1, l2, idx = (_c(t) for t in (p1, p2, lengths1, lengths2, idx))
+    ws, ws_bytes = _workspace(dev, "ball_query", N, P1, P2, K) if gp2 is not None else (None, 0)
+    _launch(dev, "ball_query_backward", _ptr(p1), _ptr(p2), N, P1, P2, _ptr(l1), _ptr(l2), K, _ptr(idx),
+            _ptr(grad_dists), _ptr(grad_nn), _ptr(ws), ws_bytes, _ptr(gp1), _ptr(gp2))
+    return gp1, gp2
+
+
 LAPLACIAN_METHODS = {"uniform": 0, "cot": 1, "cotcurv": 2}  # B200R_LAPLACIAN_*
 
 

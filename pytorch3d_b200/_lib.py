@@ -118,6 +118,12 @@ SIGNATURES = {
     "b200r_chamfer_backward": (
         ctypes.c_int,
         [_vp, _vp, _i64, _i64, _i64] + [_vp] * 5 + [_i32] * 5 + [_vp] * 8 + [_vp, _sz] + [_vp] * 3),
+    "b200r_sample_farthest_points": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp]),
+    "b200r_ball_query_workspace_bytes": (_sz, [_i64, _i64, _i64, _i64]),
+    "b200r_ball_query_forward": (
+        ctypes.c_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _i64, _f32, _i32, _vp, _vp, _vp, _vp]),
+    "b200r_ball_query_backward": (
+        ctypes.c_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
     "b200r_regularizers_workspace_bytes": (_sz, [_i64, _i64, _i32]),
     "b200r_mesh_edge_table": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _i32, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
     "b200r_mesh_edge_loss_forward": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i32, _f32, _vp, _sz, _vp, _vp]),

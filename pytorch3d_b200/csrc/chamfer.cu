@@ -21,16 +21,13 @@
 // add each point's rows in one thread, its own row first.  No float atomics, no host synchronisation.
 #include <climits>
 
-#include "bulk_copy.cuh"
-#include "mesh_tables.cuh"
+#include "point_pairs.cuh"
 
 namespace b200r {
 namespace {
 
 constexpr int kQ = 4;        // query points per thread
-constexpr int kTile = 512;   // target points per shared-memory tile
 constexpr float kCosEps = 1e-6f;  // F.cosine_similarity(..., eps=1e-6) in chamfer.py
-constexpr size_t kAlign = 256;
 
 struct NNArgs {
   const float* pts[2];     // x (N, P1, 3), y (N, P2, 3)
@@ -42,41 +39,6 @@ struct NNArgs {
   int64_t qtiles[2];       // query tiles per cloud of each direction (0: the direction is not searched)
   int64_t splits, chunk;   // the target range of split s is [s chunk, (s + 1) chunk)
 };
-
-__device__ __forceinline__ int64_t cloud_len(const int64_t* __restrict__ len, int64_t n, int64_t P) {
-  if (len == nullptr) return P;
-  const int64_t l = __ldg(len + n);
-  return l < 0 ? 0 : (l > P ? P : l);
-}
-
-// The reference's pair distance (KNearestNeighborKernelV3<float, 3, 1>, SASS of nvcc -O3 for sm_90a).
-template <int NORM>
-__device__ __forceinline__ float pair_dist(float qx, float qy, float qz, float tx, float ty, float tz) {
-  const float dx = __fsub_rn(qx, tx), dy = __fsub_rn(qy, ty), dz = __fsub_rn(qz, tz);
-  if (NORM == 2) return __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmaf_rn(dx, dx, 0.0f)));
-  return __fadd_rn(__fadd_rn(__fadd_rn(0.0f, fabsf(dx)), fabsf(dy)), fabsf(dz));
-}
-
-template <int NORM>
-__device__ __forceinline__ float dist_to(const float* __restrict__ t, int64_t j, float qx, float qy, float qz) {
-  return pair_dist<NORM>(qx, qy, qz, __ldg(t + 3 * j), __ldg(t + 3 * j + 1), __ldg(t + 3 * j + 2));
-}
-
-__device__ __forceinline__ void cp_async4(void* dst_smem, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(smem_u32(dst_smem)), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
-
-// Targets [j, j + cnt) of cloud t into buf as (x, y, z, -) float4, one 4-byte asynchronous copy per word.
-__device__ __forceinline__ void load_tile(float4* buf, const float* __restrict__ t, int64_t j, int cnt) {
-  const float* src = t + 3 * j;
-  for (int w = threadIdx.x; w < 3 * cnt; w += kThreads) {
-    const int p = w / 3, c = w - 3 * p;
-    cp_async4(reinterpret_cast<float*>(buf + p) + c, src + w);
-  }
-}
 
 template <int NORM>
 __global__ void __launch_bounds__(kThreads) nn_search_kernel(NNArgs a) {
@@ -521,14 +483,6 @@ struct Layout {
   size_t rows, nrows, ids_in;
   size_t total;
 };
-
-int64_t num_sms() {
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-      sms <= 0)
-    sms = 132;
-  return sms;
-}
 
 // The search's decomposition: query tiles per cloud, splits of the target range and their length.
 void plan(int64_t N, int64_t P1, int64_t P2, bool single, NNArgs& a) {

@@ -116,6 +116,16 @@ clouds with D = 3 on one device (tensors or Pointclouds), with int64 (N,) length
 float32 (N,) weights that do not require grad on that device, within the kernels' size limits, to
 `pytorch3d_b200.chamfer`; everything else (CPU tensors, float64, D != 3, mixed devices, weights that require grad,
 oversized inputs, and calls the reference rejects) goes to the original.
+
+`install_point_ops()` (separate again) serves PointNet++'s sample-and-group:
+    pytorch3d/ops/__init__.py                       from .sample_farthest_points import sample_farthest_points
+                                                    from .ball_query import ball_query
+    pytorch3d/ops/sample_farthest_points.py         sample_farthest_points (FarthestPointSampling, masked_gather)
+    pytorch3d/ops/ball_query.py                     ball_query (BallQuery, knn_points_backward, masked_gather)
+It replaces each function in its defining module and the name in `pytorch3d.ops` by one that sends float32 CUDA
+clouds with D = 3 and int64 (N,) lengths (or None) on their device, within the kernels' size limits, to
+`pytorch3d_b200.point_ops`; everything else (CPU tensors, float64, D != 3, mixed devices, a K the reference would
+reject, oversized inputs) goes to the original.
 """
 import importlib
 import numbers
@@ -152,7 +162,7 @@ _SHADER_MODULE = "pytorch3d.renderer.mesh.shader"
 _DEPTH_SHADERS = ("SoftDepthShader", "HardDepthShader")
 _saved = {}
 # (module name, attribute) -> original (install_blending, install_splatter, install_shading, install_gouraud,
-# install_clipping, install_normals, install_regularizers, install_sampling and install_chamfer)
+# install_clipping, install_normals, install_regularizers, install_sampling, install_chamfer and install_point_ops)
 _saved_blend = {}
 # (module name, class name, method name) -> original (install_textures, install_texture_atlas, install_normals,
 # install_depth_shading)
@@ -764,6 +774,87 @@ def install_chamfer():
     return [_LOSS_PACKAGE, _CHAMFER_MODULE]
 
 
+_FPS_MODULE = "pytorch3d.ops.sample_farthest_points"
+_BALL_MODULE = "pytorch3d.ops.ball_query"
+
+
+def _cloud_fused(points):
+    return (torch.is_tensor(points) and points.is_cuda and points.dtype == torch.float32 and points.dim() == 3
+            and points.shape[2] == 3)
+
+
+def _lengths_fused(lengths, points):
+    return lengths is None or (torch.is_tensor(lengths) and lengths.is_cuda and lengths.device == points.device
+                               and lengths.dtype == torch.int64 and tuple(lengths.shape) == (points.shape[0],))
+
+
+def _fps_fused(points, lengths, K):
+    """Whether the fused sampler takes this call: float32 CUDA (N, P, 3) points, int64 (N,) lengths (or None) on their
+    device, K an int, a list or a tensor on that device, P < 2^31."""
+    if not (_cloud_fused(points) and _lengths_fused(lengths, points)):
+        return False
+    if torch.is_tensor(K):
+        if not (K.is_cuda and K.device == points.device):
+            return False
+    elif not isinstance(K, (int, list)) or isinstance(K, bool):
+        return False
+    return _b200_C.fps_sizes_ok(int(points.shape[1]))
+
+
+def _ball_fused(p1, p2, lengths1, lengths2, K):
+    """Whether the fused ball query takes this call: float32 CUDA (N, P1, 3) and (N, P2, 3) clouds on one device,
+    int64 (N,) lengths (or None) there, an integer K >= 0, within the kernels' size limits."""
+    if not (_cloud_fused(p1) and _cloud_fused(p2) and p2.device == p1.device and p2.shape[0] == p1.shape[0]):
+        return False
+    if not (_lengths_fused(lengths1, p1) and _lengths_fused(lengths2, p1)):
+        return False
+    if not isinstance(K, numbers.Integral) or isinstance(K, bool):
+        return False
+    return _b200_C.ball_query_sizes_ok(int(p1.shape[0]), int(p1.shape[1]), int(p2.shape[1]), int(K))
+
+
+def _fps_dispatch(original):
+    from . import point_ops as ours
+
+    def sample_farthest_points(points, lengths=None, K=50, random_start_point: bool = False):
+        if _fps_fused(points, lengths, K):
+            return ours.sample_farthest_points(points, lengths, K, random_start_point)
+        return original(points, lengths, K, random_start_point)
+
+    sample_farthest_points.__doc__ = original.__doc__
+    return sample_farthest_points
+
+
+def _ball_dispatch(original):
+    from . import point_ops as ours
+
+    def ball_query(p1, p2, lengths1=None, lengths2=None, K: int = 500, radius: float = 0.2, return_nn: bool = True,
+                   skip_points_outside_cube: bool = False):
+        args = (p1, p2, lengths1, lengths2, K, radius, return_nn, skip_points_outside_cube)
+        if _ball_fused(p1, p2, lengths1, lengths2, K):
+            return ours.ball_query(*args)
+        return original(*args)
+
+    ball_query.__doc__ = original.__doc__
+    return ball_query
+
+
+def install_point_ops():
+    """Patch PyTorch3D's point sampling and grouping (must be importable): `sample_farthest_points` in
+    pytorch3d.ops.sample_farthest_points and in pytorch3d.ops, and `ball_query` in pytorch3d.ops.ball_query and in
+    pytorch3d.ops.  Returns the list of patched module names."""
+    package = importlib.import_module(_OPS_PACKAGE)
+    for modname, name, dispatch in ((_FPS_MODULE, "sample_farthest_points", _fps_dispatch),
+                                    (_BALL_MODULE, "ball_query", _ball_dispatch)):
+        module = importlib.import_module(modname)  # the package's attribute of this name is the function
+        original = module.__dict__[name]
+        for owner, key in ((module, modname), (package, _OPS_PACKAGE)):
+            if (key, name) not in _saved_blend:
+                _saved_blend[(key, name)] = owner.__dict__[name]
+                setattr(owner, name, dispatch(original))
+    return [_OPS_PACKAGE, _FPS_MODULE, _BALL_MODULE]
+
+
 def _depth_fragments_fused(fragments, soft):
     """int64 CUDA pix_to_face (N, H, W, K) with 1 <= K <= 150, and float32 zbuf (and dists) of its shape on its device."""
     p2f = getattr(fragments, "pix_to_face", None)
@@ -827,7 +918,8 @@ def install_depth_shading():
 def uninstall():
     """Undo `install()`, `install_blending()`, `install_splatter()`, `install_shading()`, `install_gouraud()`,
     `install_textures()`, `install_texture_atlas()`, `install_clipping()`, `install_normals()`,
-    `install_regularizers()`, `install_depth_shading()`, `install_sampling()` and `install_chamfer()`."""
+    `install_regularizers()`, `install_depth_shading()`, `install_sampling()`, `install_chamfer()` and
+    `install_point_ops()`."""
     import importlib
     for modname, original in list(_saved.items()):
         importlib.import_module(modname)._C = original
