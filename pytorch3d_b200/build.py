@@ -15,7 +15,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libb200raster.so")
 SOURCES = ["raster_meshes.cu", "raster_points.cu", "compositing.cu", "blending.cu", "splatter_blend.cu", "shading.cu", "textures.cu", "texture_atlas.cu", "normals.cu", "regularizers.cu", "sampling.cu", "chamfer.cu", "point_ops.cu", "clip.cu", "interp_face_attrs.cu", "peer_exchange.cu",
            "coarse_hooks.cu", "host_api.cu"]
-HEADERS = ["raster_math.cuh", "bulk_copy.cuh", "binning.cuh", "common.cuh", "mesh_tables.cuh", "point_pairs.cuh", os.path.join("..", "..", "include", "b200_raster.h")]
+HEADERS = ["raster_math.cuh", "bulk_copy.cuh", "binning.cuh", "common.cuh", "keyed_runs.cuh", "mesh_tables.cuh", "point_pairs.cuh", os.path.join("..", "..", "include", "b200_raster.h")]
 
 
 # The one architecture the library is built for (H100, sm_90a); tools/variant_time.py builds its variants with it too.

@@ -17,8 +17,8 @@
 //      thread over the batch, which also sets the status word of the data-dependent checks.
 //
 // Backward: one thread per query point writes a gradient row for its own coordinates and one for its neighbour's
-// (and the same two for the normals), keyed by point; a stable radix sort and the segmented sum of mesh_tables.cuh
-// add each point's rows in one thread, its own row first.  No float atomics, no host synchronisation.
+// (and the same two for the normals), keyed by point; sort_into_runs and the segmented sum of keyed_runs.cuh add
+// each point's rows in one thread, its own row first.  No float atomics, no host synchronisation.
 #include <climits>
 
 #include "point_pairs.cuh"
@@ -505,24 +505,25 @@ void plan(int64_t N, int64_t P1, int64_t P2, bool single, NNArgs& a) {
 
 bool layout(int64_t N, int64_t P1, int64_t P2, int32_t pass, Layout& L) {
   L = Layout{};
+  Carver c;
   if (pass == 0) {
-    L.key0 = 0;
-    L.key1 = align_up(sizeof(unsigned long long) * (size_t)(N * P1), kAlign);
-    L.total = L.key1 + align_up(sizeof(unsigned long long) * (size_t)(N * P2), kAlign);
+    L.key0 = c.take(sizeof(unsigned long long) * (size_t)(N * P1));
+    L.key1 = c.take(sizeof(unsigned long long) * (size_t)(N * P2));
+    L.total = c.used;
     return true;
   }
   const size_t V = (size_t)(N * P1 + N * P2), R = 2 * V;
-  L.rows = 0;
-  L.nrows = L.rows + align_up(sizeof(float) * 3 * R, kAlign);
-  L.keys_in = L.nrows + align_up(sizeof(float) * 3 * R, kAlign);
-  L.keys_out = L.keys_in + align_up(sizeof(uint32_t) * R, kAlign);
-  L.ids_in = L.keys_out + align_up(sizeof(uint32_t) * R, kAlign);
-  L.ids_out = L.ids_in + align_up(sizeof(int32_t) * R, kAlign);
-  L.offsets = L.ids_out + align_up(sizeof(int32_t) * R, kAlign);
-  L.cub = L.offsets + align_up(sizeof(int32_t) * (V + 1), kAlign);
-  if (!corner_sort_bytes((int64_t)V, R, L.cub_bytes)) return false;
-  L.total = L.cub + align_up(L.cub_bytes, kAlign);
-  return true;
+  L.rows = c.take(sizeof(float) * 3 * R);
+  L.nrows = c.take(sizeof(float) * 3 * R);
+  L.keys_in = c.take(sizeof(uint32_t) * R);
+  L.keys_out = c.take(sizeof(uint32_t) * R);
+  L.ids_in = c.take(sizeof(int32_t) * R);
+  L.ids_out = c.take(sizeof(int32_t) * R);
+  L.offsets = c.take(sizeof(int32_t) * (V + 1));
+  const bool sized = run_sort_bytes((int64_t)V, (int64_t)R, L.cub_bytes);
+  L.cub = c.take(L.cub_bytes);
+  L.total = c.used;
+  return sized;
 }
 
 int check_args(const char* op, int64_t N, int64_t P1, int64_t P2, int32_t norm, int32_t point_red, int32_t batch_red) {
@@ -573,11 +574,8 @@ using namespace b200r;
 extern "C" size_t b200r_chamfer_workspace_bytes(int64_t N, int64_t P1, int64_t P2, int32_t pass) {
   if (N < 1 || P1 < 1 || P2 < 1 || (pass != 0 && pass != 1)) return 0;
   Layout L;
-  if (!layout(N, P1, P2, pass, L)) {
-    cudaGetLastError();
-    return 0;
-  }
-  return L.total;
+  const bool sized = layout(N, P1, P2, pass, L);
+  return workspace_size(sized, L.total);
 }
 
 extern "C" int b200r_chamfer_forward(const float* x, const float* y, int64_t N, int64_t P1, int64_t P2,
@@ -591,7 +589,7 @@ extern "C" int b200r_chamfer_forward(const float* x, const float* y, int64_t N, 
   int rc = check_args("chamfer_forward", N, P1, P2, norm, point_red, batch_red);
   if (rc != B200R_OK) return rc;
   Layout L;
-  if (!layout(N, P1, P2, 0, L)) return fail(B200R_ERR_CUDA, "chamfer_forward: could not size the workspace");
+  layout(N, P1, P2, 0, L);  // the forward's keys need no cub storage
   NNArgs s{};
   plan(N, P1, P2, single != 0, s);
   if (s.splits > 1 && (workspace == nullptr || workspace_bytes < L.total))
@@ -652,12 +650,9 @@ extern "C" int b200r_chamfer_backward(const float* x, const float* y, int64_t N,
   if (grad_normals != nullptr && (x_normals == nullptr || y_normals == nullptr || grad_nx == nullptr))
     return fail(B200R_ERR_INVALID_ARGUMENT, "chamfer_backward: the normals' gradient needs the normals and theirs");
   Layout L;
-  if (!layout(N, P1, P2, 1, L)) {
-    cudaGetLastError();
-    return fail(B200R_ERR_CUDA, "chamfer_backward: cub could not size the sort's temporary storage");
-  }
-  if (workspace == nullptr || workspace_bytes < L.total)
-    return fail(B200R_ERR_INVALID_ARGUMENT, "chamfer_backward: workspace smaller than b200r_chamfer_workspace_bytes");
+  const bool sized = layout(N, P1, P2, 1, L);
+  rc = check_workspace("chamfer_backward", "b200r_chamfer_workspace_bytes", sized, L.total, workspace, workspace_bytes);
+  if (rc != B200R_OK) return rc;
   char* ws = static_cast<char*>(workspace);
   GradArgs g{};
   g.f = loss_args(x, y, N, P1, P2, x_lengths, y_lengths, x_normals, y_normals, weights, point_red, batch_red, single,
@@ -677,19 +672,16 @@ extern "C" int b200r_chamfer_backward(const float* x, const float* y, int64_t N,
   const int64_t V = N * P1 + N * P2, R = 2 * V;
   grad_rows_kernel<<<grid_for(V), kThreads, 0, stream>>>(g);
   B200R_LAUNCHED("grad_rows_kernel");
-  B200R_CUDA_OK(cub::DeviceRadixSort::SortPairs(ws + L.cub, L.cub_bytes, g.keys, keys_out, g.ids, ids_out, (int)R, 0,
-                                                key_bits(V), stream));
-  run_offsets_kernel<<<grid_for(R + 1), kThreads, 0, stream>>>(keys_out, R, V, offsets);
-  B200R_LAUNCHED("run_offsets_kernel");
-  // row ids are < R: segmented_sum_kernel's (j, f) decoding with F = R gives j = 0, f = id
+  rc = sort_into_runs(g.keys, keys_out, g.ids, ids_out, R, V, ws + L.cub, L.cub_bytes, offsets, stream);
+  if (rc != B200R_OK) return rc;
   if (grad_points != nullptr) {
-    segmented_sum_kernel<RowOf::kFace, Epilogue::kSum>
-        <<<grid_for(V), kThreads, 0, stream>>>(offsets, ids_out, V, R, g.rows, nullptr, grad_points);
+    segmented_sum_kernel<Mode::kSum>
+        <<<grid_for(V), kThreads, 0, stream>>>(offsets, ids_out, V, RowsById{{}, g.rows}, nullptr, grad_points);
     B200R_LAUNCHED("segmented_sum_kernel");
   }
   if (grad_normals != nullptr) {
-    segmented_sum_kernel<RowOf::kFace, Epilogue::kSum>
-        <<<grid_for(V), kThreads, 0, stream>>>(offsets, ids_out, V, R, g.nrows, nullptr, grad_normals);
+    segmented_sum_kernel<Mode::kSum>
+        <<<grid_for(V), kThreads, 0, stream>>>(offsets, ids_out, V, RowsById{{}, g.nrows}, nullptr, grad_normals);
     B200R_LAUNCHED("segmented_sum_kernel");
   }
   return B200R_OK;

@@ -78,13 +78,19 @@ inline cudaError_t launch_chained(void (*kernel)(KArgs...), dim3 grid, dim3 bloc
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-// Grid-stride kernels launch at most 32 CTAs per SM of the current device: more would only queue behind resident ones.
-inline int64_t cap_grid_stride_blocks(int64_t blocks) {
+// The current device's SM count, the launch plans' measure of a full device (132 on an H100 SXM when it cannot be read).
+inline int64_t num_sms() {
   int dev = 0, sms = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
       sms <= 0)
-    sms = 132;  // H100 SXM
-  return blocks < (int64_t)sms * 32 ? blocks : (int64_t)sms * 32;
+    sms = 132;
+  return sms;
+}
+
+// Grid-stride kernels launch at most 32 CTAs per SM of the current device: more would only queue behind resident ones.
+inline int64_t cap_grid_stride_blocks(int64_t blocks) {
+  const int64_t cap = num_sms() * 32;
+  return blocks < cap ? blocks : cap;
 }
 
 inline int div_up(int a, int b) { return (a + b - 1) / b; }

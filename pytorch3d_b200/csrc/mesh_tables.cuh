@@ -1,22 +1,16 @@
-// Mesh topology tables shared by the normals (normals.cu, DESIGN.md section 17), the mesh regularisers
-// (regularizers.cu, section 18) and the surface sampler (sampling.cu, section 20): the vertex -> corner table, the one
-// segmented sum over it, and the face-area and normalisation arithmetic they have in common.
+// Mesh arithmetic shared by the normals (normals.cu, DESIGN.md section 17), the mesh regularisers (regularizers.cu,
+// section 18) and the surface sampler (sampling.cu, section 20): the face corners, the face-area and normalisation
+// arithmetic, and the vertex -> corner table.
 //
-// Corner j of face f has the id c = j * F + f and the key faces[f, j]; a stable radix sort of the 3F (key, id) pairs
-// over key_bits(V) bits, and an offset array of V + 1 entries, give every vertex the run of its corners in (j, f)
-// order.  Every per-vertex sum is one thread walking its run from +0 with __fadd_rn, so there are no float atomics and
-// the results do not depend on scheduling.
+// Corner j of face f has the id c = j * F + f and the key faces[f, j]; sort_into_runs (keyed_runs.cuh) over the 3F
+// (key, id) pairs gives every vertex the run of its corners in (j, f) order, and segmented_sum_kernel sums a per-face
+// or per-corner row over it.
 #pragma once
 
-#include <cub/device/device_radix_sort.cuh>
-
-#include "common.cuh"
+#include "keyed_runs.cuh"
 
 namespace b200r {
 namespace {
-
-constexpr int kThreads = 256;
-constexpr float kNormalizeEps = 1e-6f;  // F.normalize(..., eps=1e-6) in Meshes._compute_vertex_normals
 
 // The three corners of face f.  A face index outside [0, V) (the reference does not check them either) gives NaN
 // corners instead of a read out of bounds.
@@ -39,11 +33,6 @@ __device__ __forceinline__ void face_corners(const float* __restrict__ verts, co
 __device__ __forceinline__ float3 cross_fma(float3 a, float3 b) {
   return make_float3(__fmaf_rn(a.y, b.z, -__fmul_rn(a.z, b.y)), __fmaf_rn(a.z, b.x, -__fmul_rn(a.x, b.z)),
                      __fmaf_rn(a.x, b.y, -__fmul_rn(a.y, b.x)));
-}
-
-// |s| as torch's 2-norm over dim 1 of a float32 (V, 3) tensor computes it.
-__device__ __forceinline__ float norm3(float3 s) {
-  return __fsqrt_rn(__fmaf_rn(s.z, s.z, __fmaf_rn(s.y, s.y, __fmul_rn(s.x, s.x))));
 }
 
 __device__ __forceinline__ float3 sub_rn(float3 a, float3 b) {
@@ -78,16 +67,6 @@ __device__ __forceinline__ float3 normalize_backward(float3 s, float3 g, float e
                      __fadd_rn(__fdiv_rn(g.z, m), __fmul_rn(s.z, k)));
 }
 
-__device__ __forceinline__ float3 load3(const float* __restrict__ p, int64_t i) {
-  return make_float3(__ldg(p + 3 * i + 0), __ldg(p + 3 * i + 1), __ldg(p + 3 * i + 2));
-}
-
-__device__ __forceinline__ void store3(float* __restrict__ p, int64_t i, float3 v) {
-  p[3 * i + 0] = v.x;
-  p[3 * i + 1] = v.y;
-  p[3 * i + 2] = v.z;
-}
-
 // ---- the vertex -> corner table ---------------------------------------------------------------------------------
 
 // (key, corner id) of every corner; a face index outside [0, V) gets the key V, which sorts after every vertex and
@@ -107,87 +86,29 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 
-// offsets[v] = the first sorted position whose key is >= v, for v in [0, V]: position i writes the offsets of the
-// vertices after the previous key up to its own (the end, n, stands for the key V).
-__global__ void __launch_bounds__(kThreads)
-    run_offsets_kernel(const uint32_t* __restrict__ keys, int64_t n, int64_t V, int32_t* __restrict__ offsets) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += stride) {
-    const int64_t prev = i > 0 ? (int64_t)keys[i - 1] : -1;
-    const int64_t cur = i < n ? (int64_t)keys[i] : V;
-    for (int64_t v = prev + 1; v <= cur; ++v) offsets[v] = (int32_t)i;
+// Rows of corner ids c = j * n + i (i < n, j < 3): rows[i] of (n, 3) per item, or rows[i * 3 + j] of (n, 3, 3) per
+// corner.  The items are faces, or the sampler's samples.
+template <bool PER_CORNER>
+struct CornerRows : AddedRows {
+  const float* rows;
+  int64_t n;
+  __device__ float3 operator()(int64_t, int32_t c) const {
+    const int64_t j = c >= 2 * n ? 2 : (c >= n ? 1 : 0), i = c - j * n;
+    return load3(rows, PER_CORNER ? i * 3 + j : i);
   }
-}
-
-// ---- the one segmented sum --------------------------------------------------------------------------------------
-
-enum class RowOf { kFace, kCorner };   // rows[f] (F, 3) or rows[f * 3 + j] (F, 3, 3)
-enum class Epilogue { kSum, kNormalize };
-
-// Per vertex: the sum of its corners' rows in run order from +0.  kNormalize also stores the sum in `sums` and writes
-// sum / max(|sum|, 1e-6) to `out`.
-template <RowOf ROW, Epilogue EPI>
-__global__ void __launch_bounds__(kThreads)
-    segmented_sum_kernel(const int32_t* __restrict__ offsets, const int32_t* __restrict__ corners, int64_t V,
-                         int64_t F, const float* __restrict__ rows, float* __restrict__ sums,
-                         float* __restrict__ out) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < V; v += stride) {
-    const int32_t end = __ldg(offsets + v + 1);
-    float3 acc = make_float3(0.0f, 0.0f, 0.0f);
-    for (int32_t i = __ldg(offsets + v); i < end; ++i) {
-      const int64_t c = __ldg(corners + i);
-      const int64_t j = c >= 2 * F ? 2 : (c >= F ? 1 : 0);
-      const int64_t f = c - j * F;
-      const float3 r = load3(rows, ROW == RowOf::kFace ? f : f * 3 + j);
-      acc = make_float3(__fadd_rn(acc.x, r.x), __fadd_rn(acc.y, r.y), __fadd_rn(acc.z, r.z));
-    }
-    if (EPI == Epilogue::kNormalize) {
-      store3(sums, v, acc);
-      const float n = norm3(acc);
-      const float m = n < kNormalizeEps ? kNormalizeEps : n;  // clamp_min: NaN stays NaN
-      acc = make_float3(__fdiv_rn(acc.x, m), __fdiv_rn(acc.y, m), __fdiv_rn(acc.z, m));
-    }
-    store3(out, v, acc);
-  }
-}
+};
 
 // ---- host side ----------------------------------------------------------------------------------------------------
 
-// ceil(log2(V + 1)): the key bits the sort looks at (the key V, for faces out of range, included).
-int key_bits(int64_t V) {
-  int bits = 1;
-  while (bits < 32 && (V >> bits) != 0) ++bits;
-  return bits;
-}
-
-dim3 grid_for(int64_t n) { return dim3((unsigned)cap_grid_stride_blocks((n + kThreads - 1) / kThreads)); }
-
-// cub's temporary storage for sorting n (uint32 key, int32 id) pairs over key_bits(V) bits; false when cub cannot size
-// it (no device).
-bool corner_sort_bytes(int64_t V, size_t n, size_t& bytes) {
-  bytes = 0;
-  return n == 0 || cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
-                                                   (const int32_t*)nullptr, (int32_t*)nullptr, (int)n, 0,
-                                                   key_bits(V)) == cudaSuccess;
-}
-
 // Builds the vertex -> corner table (offsets[V + 1], then the 3F corner ids in run order) at `table`, with keys_in,
-// keys_out and ids_in of 3F entries and cub's storage of corner_sort_bytes(V, 3F) bytes as scratch.
+// keys_out and ids_in of 3F entries and cub's storage of run_sort_bytes(V, 3F) bytes as scratch.
 int build_table(const int64_t* faces, int64_t V, int64_t F, uint32_t* keys_in, uint32_t* keys_out, int32_t* ids_in,
                 void* cub_storage, size_t cub_bytes, int32_t* table, cudaStream_t stream) {
-  const int64_t n = 3 * F;
-  int32_t* offsets = table;
-  int32_t* corners = table + V + 1;
-  if (n > 0) {
+  if (F > 0) {
     corner_keys_kernel<<<grid_for(F), kThreads, 0, stream>>>(faces, F, V, keys_in, ids_in);
     B200R_LAUNCHED("corner_keys_kernel");
-    B200R_CUDA_OK(cub::DeviceRadixSort::SortPairs(cub_storage, cub_bytes, keys_in, keys_out, ids_in, corners, (int)n,
-                                                  0, key_bits(V), stream));
   }
-  run_offsets_kernel<<<grid_for(n + 1), kThreads, 0, stream>>>(keys_out, n, V, offsets);
-  B200R_LAUNCHED("run_offsets_kernel");
-  return B200R_OK;
+  return sort_into_runs(keys_in, keys_out, ids_in, table + V + 1, 3 * F, V, cub_storage, cub_bytes, table, stream);
 }
 
 }  // namespace

@@ -1,6 +1,6 @@
 // Mesh normals: vertex normals and face areas / normals, forward and deterministic backward (DESIGN.md section 17).
 //
-// Both ops rest on one structure, the vertex -> corner table (mesh_tables.cuh).  Corner j of face f has the id
+// Both ops rest on one structure, the vertex -> corner table (mesh_tables.cuh, keyed_runs.cuh).  Corner j of face f has the id
 // c = j * F + f and the key faces[f, j]; a stable radix sort of the 3F (key, id) pairs over ceil(log2(V + 1)) key bits,
 // and an offset array of V + 1 entries, give every vertex the run of its corners in (j, f) order.  That is the order in
 // which the three serial index_add calls of pytorch3d/structures/meshes.py Meshes._compute_vertex_normals accumulate on
@@ -24,8 +24,6 @@
 
 namespace b200r {
 namespace {
-
-constexpr size_t kAlign = 256;
 
 // ---- vertex normals -----------------------------------------------------------------------------------------------
 
@@ -163,15 +161,16 @@ struct Layout {
 
 bool layout(int64_t V, int64_t F, Layout& L) {
   const size_t n = 3 * (size_t)F;
-  L.rows = 0;
-  L.table = L.rows + align_up(sizeof(float) * 9 * (size_t)F, kAlign);
-  L.keys_in = L.table + align_up(sizeof(int32_t) * ((size_t)V + 1 + n), kAlign);
-  L.keys_out = L.keys_in + align_up(sizeof(uint32_t) * n, kAlign);
-  L.ids_in = L.keys_out + align_up(sizeof(uint32_t) * n, kAlign);
-  L.cub = L.ids_in + align_up(sizeof(int32_t) * n, kAlign);
-  if (!corner_sort_bytes(V, n, L.cub_bytes)) return false;
-  L.total = L.cub + align_up(L.cub_bytes, kAlign);
-  return true;
+  Carver c;
+  L.rows = c.take(sizeof(float) * 9 * (size_t)F);
+  L.table = c.take(sizeof(int32_t) * ((size_t)V + 1 + n));
+  L.keys_in = c.take(sizeof(uint32_t) * n);
+  L.keys_out = c.take(sizeof(uint32_t) * n);
+  L.ids_in = c.take(sizeof(int32_t) * n);
+  const bool sized = run_sort_bytes(V, (int64_t)n, L.cub_bytes);
+  L.cub = c.take(L.cub_bytes);
+  L.total = c.used;
+  return sized;
 }
 
 int check_sizes(const char* op, int64_t V, int64_t F) {
@@ -184,13 +183,8 @@ int check_sizes(const char* op, int64_t V, int64_t F) {
 }
 
 int checked_layout(const char* op, int64_t V, int64_t F, size_t workspace_bytes, const void* workspace, Layout& L) {
-  if (!layout(V, F, L)) {
-    cudaGetLastError();
-    return fail(B200R_ERR_CUDA, std::string(op) + ": cub could not size the sort's temporary storage");
-  }
-  if (workspace == nullptr || workspace_bytes < L.total)
-    return fail(B200R_ERR_INVALID_ARGUMENT, std::string(op) + ": workspace smaller than b200r_normals_workspace_bytes");
-  return B200R_OK;
+  const bool sized = layout(V, F, L);
+  return check_workspace(op, "b200r_normals_workspace_bytes", sized, L.total, workspace, workspace_bytes);
 }
 
 // Builds the table (offsets[V + 1], then the 3F corner ids in run order) at `table`.
@@ -209,11 +203,8 @@ using namespace b200r;
 extern "C" size_t b200r_normals_workspace_bytes(int64_t V, int64_t F) {
   if (V < 0 || F < 0) return 0;
   Layout L;
-  if (!layout(V, F, L)) {
-    cudaGetLastError();
-    return 0;
-  }
-  return L.total;
+  const bool sized = layout(V, F, L);
+  return workspace_size(sized, L.total);
 }
 
 extern "C" int b200r_verts_normals_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F,
@@ -234,8 +225,8 @@ extern "C" int b200r_verts_normals_forward(const float* verts, int64_t V, const 
     face_normal_rows_kernel<<<grid_for(F), kThreads, 0, stream>>>(verts, faces, V, F, rows);
     B200R_LAUNCHED("face_normal_rows_kernel");
   }
-  segmented_sum_kernel<RowOf::kFace, Epilogue::kNormalize>
-      <<<grid_for(V), kThreads, 0, stream>>>(table, table + V + 1, V, F, rows, sums, normals);
+  segmented_sum_kernel<Mode::kNormalize>
+      <<<grid_for(V), kThreads, 0, stream>>>(table, table + V + 1, V, CornerRows<false>{{}, rows, F}, sums, normals);
   B200R_LAUNCHED("segmented_sum_kernel");
   return B200R_OK;
 }
@@ -260,8 +251,8 @@ extern "C" int b200r_verts_normals_backward(const float* grad_normals, const flo
     cross_backward_rows_kernel<<<grid_for(F), kThreads, 0, stream>>>(verts, faces, V, F, grad_sums, rows);
     B200R_LAUNCHED("cross_backward_rows_kernel");
   }
-  segmented_sum_kernel<RowOf::kCorner, Epilogue::kSum>
-      <<<grid_for(V), kThreads, 0, stream>>>(table, table + V + 1, V, F, rows, nullptr, grad_verts);
+  segmented_sum_kernel<Mode::kSum>
+      <<<grid_for(V), kThreads, 0, stream>>>(table, table + V + 1, V, CornerRows<true>{{}, rows, F}, nullptr, grad_verts);
   B200R_LAUNCHED("segmented_sum_kernel");
   return B200R_OK;
 }
@@ -298,8 +289,8 @@ extern "C" int b200r_face_areas_normals_backward(const float* grad_areas, const 
                                                                                   faces, V, F, rows);
     B200R_LAUNCHED("face_areas_normals_backward_rows_kernel");
   }
-  segmented_sum_kernel<RowOf::kCorner, Epilogue::kSum>
-      <<<grid_for(V), kThreads, 0, stream>>>(table, table + V + 1, V, F, rows, nullptr, grad_verts);
+  segmented_sum_kernel<Mode::kSum>
+      <<<grid_for(V), kThreads, 0, stream>>>(table, table + V + 1, V, CornerRows<true>{{}, rows, F}, nullptr, grad_verts);
   B200R_LAUNCHED("segmented_sum_kernel");
   return B200R_OK;
 }

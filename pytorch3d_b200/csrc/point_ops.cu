@@ -23,8 +23,8 @@
 // written afterwards in coalesced stores, so every output element is written once.
 //
 // Ball query backward: one thread per query sums its hits' rows 2 g (p1 - p2) in k order into grad_p1; grad_p2 is, per
-// target, the sum of -2 g (p1 - p2) + g_nn over its hits in (i, k) order: a stable radix sort of the hits by target
-// (mesh_tables.cuh) and a segmented sum that recomputes each row from its id, in chunks of at most kBallChunk rows, each
+// target, the sum of -2 g (p1 - p2) + g_nn over its hits in (i, k) order: sort_into_runs over the hits by target and
+// segmented_sum_kernel (keyed_runs.cuh) with a row recomputed from its id, in chunks of at most kBallChunk rows, each
 // chunk continuing the previous chunk's sums.  No float atomics, no (N, P2, K, 3) buffer, no host synchronisation.
 #include <cooperative_groups.h>
 
@@ -339,30 +339,22 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 
-// grad_p2[v] (+)= the rows of v's run in order: -diff + g_nn, each recomputed from its row id.
-__global__ void __launch_bounds__(kThreads)
-    ball_segment_kernel(BallGradArgs a, int64_t r0, int first, const int32_t* __restrict__ offsets,
-                        const int32_t* __restrict__ ids, float* __restrict__ grad_p2) {
-  const int64_t V = a.N * a.P2, stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < V; v += stride) {
-    const int32_t end = __ldg(offsets + v + 1);
-    int32_t s = __ldg(offsets + v);
-    if (!first && s == end) continue;
-    float3 acc = first ? make_float3(0.0f, 0.0f, 0.0f) : load3(grad_p2, v);
-    const float3 tp = load3(a.p2, v);
-    for (; s < end; ++s) {
-      const int64_t r = r0 + __ldg(ids + s), q = r / a.K;
-      const float3 d = ball_diff(a, r, load3(a.p1, q), tp);
-      float3 row = make_float3(-d.x, -d.y, -d.z);
-      if (a.gnn != nullptr) {
-        const float3 g = load3(a.gnn, r);
-        row = make_float3(__fadd_rn(row.x, g.x), __fadd_rn(row.y, g.y), __fadd_rn(row.z, g.z));
-      }
-      acc = make_float3(__fadd_rn(acc.x, row.x), __fadd_rn(acc.y, row.y), __fadd_rn(acc.z, row.z));
+// The grad_p2 row of hit r0 + id at target point tp: -diff + g_nn, recomputed from the row.
+struct BallRow : AddedRows {
+  BallGradArgs a;
+  int64_t r0;
+  __device__ float3 at_key(int64_t v) const { return load3(a.p2, v); }
+  __device__ float3 operator()(float3 tp, int32_t id) const {
+    const int64_t r = r0 + id, q = r / a.K;
+    const float3 d = ball_diff(a, r, load3(a.p1, q), tp);
+    float3 row = make_float3(-d.x, -d.y, -d.z);
+    if (a.gnn != nullptr) {
+      const float3 g = load3(a.gnn, r);
+      row = make_float3(__fadd_rn(row.x, g.x), __fadd_rn(row.y, g.y), __fadd_rn(row.z, g.z));
     }
-    store3(grad_p2, v, acc);
+    return row;
   }
-}
+};
 
 // ---- host side ------------------------------------------------------------------------------------------------------
 
@@ -428,15 +420,16 @@ bool ball_layout(int64_t N, int64_t P1, int64_t P2, int64_t K, BallLayout& L) {
   const int64_t R = N * P1 * K, V = N * P2;
   L.chunk = R < kBallChunk ? R : kBallChunk;
   const size_t c = (size_t)(L.chunk > 0 ? L.chunk : 1);
-  L.keys_in = 0;
-  L.keys_out = L.keys_in + align_up(sizeof(uint32_t) * c, kAlign);
-  L.ids_in = L.keys_out + align_up(sizeof(uint32_t) * c, kAlign);
-  L.ids_out = L.ids_in + align_up(sizeof(int32_t) * c, kAlign);
-  L.offsets = L.ids_out + align_up(sizeof(int32_t) * c, kAlign);
-  L.cub = L.offsets + align_up(sizeof(int32_t) * (size_t)(V + 1), kAlign);
-  if (!corner_sort_bytes(V, c, L.cub_bytes)) return false;
-  L.total = L.cub + align_up(L.cub_bytes, kAlign);
-  return true;
+  Carver w;
+  L.keys_in = w.take(sizeof(uint32_t) * c);
+  L.keys_out = w.take(sizeof(uint32_t) * c);
+  L.ids_in = w.take(sizeof(int32_t) * c);
+  L.ids_out = w.take(sizeof(int32_t) * c);
+  L.offsets = w.take(sizeof(int32_t) * (size_t)(V + 1));
+  const bool sized = run_sort_bytes(V, (int64_t)c, L.cub_bytes);
+  L.cub = w.take(L.cub_bytes);
+  L.total = w.used;
+  return sized;
 }
 
 int check_ball(const char* op, int64_t N, int64_t P1, int64_t P2, int64_t K) {
@@ -475,11 +468,8 @@ extern "C" int b200r_sample_farthest_points(const float* points, int64_t N, int6
 extern "C" size_t b200r_ball_query_workspace_bytes(int64_t N, int64_t P1, int64_t P2, int64_t K) {
   if (check_ball("ball_query", N, P1, P2, K) != B200R_OK) return 0;
   BallLayout L;
-  if (!ball_layout(N, P1, P2, K, L)) {
-    cudaGetLastError();
-    return 0;
-  }
-  return L.total;
+  const bool sized = ball_layout(N, P1, P2, K, L);
+  return workspace_size(sized, L.total);
 }
 
 extern "C" int b200r_ball_query_forward(const float* p1, const float* p2, int64_t N, int64_t P1, int64_t P2,
@@ -532,13 +522,10 @@ extern "C" int b200r_ball_query_backward(const float* p1, const float* p2, int64
     return B200R_OK;
   }
   BallLayout L;
-  if (!ball_layout(N, P1, P2, K, L)) {
-    cudaGetLastError();
-    return fail(B200R_ERR_CUDA, "ball_query_backward: cub could not size the sort's temporary storage");
-  }
-  if (workspace == nullptr || workspace_bytes < L.total)
-    return fail(B200R_ERR_INVALID_ARGUMENT,
-                "ball_query_backward: workspace smaller than b200r_ball_query_workspace_bytes");
+  const bool sized = ball_layout(N, P1, P2, K, L);
+  rc = check_workspace("ball_query_backward", "b200r_ball_query_workspace_bytes", sized, L.total, workspace,
+                       workspace_bytes);
+  if (rc != B200R_OK) return rc;
   char* ws = static_cast<char*>(workspace);
   uint32_t* keys_in = reinterpret_cast<uint32_t*>(ws + L.keys_in);
   uint32_t* keys_out = reinterpret_cast<uint32_t*>(ws + L.keys_out);
@@ -549,12 +536,15 @@ extern "C" int b200r_ball_query_backward(const float* p1, const float* p2, int64
     const int64_t cnt = R - r0 < L.chunk ? R - r0 : L.chunk;
     ball_keys_kernel<<<grid_for(cnt), kThreads, 0, stream>>>(a, r0, cnt, keys_in, ids_in);
     B200R_LAUNCHED("ball_keys_kernel");
-    B200R_CUDA_OK(cub::DeviceRadixSort::SortPairs(ws + L.cub, L.cub_bytes, keys_in, keys_out, ids_in, ids_out,
-                                                  (int)cnt, 0, key_bits(V), stream));
-    run_offsets_kernel<<<grid_for(cnt + 1), kThreads, 0, stream>>>(keys_out, cnt, V, offsets);
-    B200R_LAUNCHED("run_offsets_kernel");
-    ball_segment_kernel<<<grid_for(V), kThreads, 0, stream>>>(a, r0, r0 == 0, offsets, ids_out, grad_p2);
-    B200R_LAUNCHED("ball_segment_kernel");
+    rc = sort_into_runs(keys_in, keys_out, ids_in, ids_out, cnt, V, ws + L.cub, L.cub_bytes, offsets, stream);
+    if (rc != B200R_OK) return rc;
+    if (r0 == 0)
+      segmented_sum_kernel<Mode::kSum>
+          <<<grid_for(V), kThreads, 0, stream>>>(offsets, ids_out, V, BallRow{{}, a, r0}, nullptr, grad_p2);
+    else
+      segmented_sum_kernel<Mode::kContinue>
+          <<<grid_for(V), kThreads, 0, stream>>>(offsets, ids_out, V, BallRow{{}, a, r0}, nullptr, grad_p2);
+    B200R_LAUNCHED("segmented_sum_kernel");
   }
   return B200R_OK;
 }

@@ -1,15 +1,14 @@
-// The point-pair arithmetic, the target-tile stream and the host helpers shared by the point-cloud ops: chamfer
+// The point-pair arithmetic and the target-tile stream shared by the point-cloud ops: chamfer
 // distance (chamfer.cu, DESIGN.md section 21) and farthest point sampling and ball query (point_ops.cu, section 22).
 #pragma once
 
 #include "bulk_copy.cuh"
-#include "mesh_tables.cuh"
+#include "keyed_runs.cuh"
 
 namespace b200r {
 namespace {
 
 constexpr int kTile = 512;  // target points per shared-memory tile
-constexpr size_t kAlign = 256;  // workspace sub-array alignment
 
 // lengths[n] clamped to [0, P]; P when there are no lengths.
 __device__ __forceinline__ int64_t cloud_len(const int64_t* __restrict__ len, int64_t n, int64_t P) {
@@ -47,15 +46,6 @@ __device__ __forceinline__ void load_tile(float4* buf, const float* __restrict__
     const int p = w / 3, c = w - 3 * p;
     cp_async4(reinterpret_cast<float*>(buf + p) + c, src + w);
   }
-}
-
-// The current device's SM count, the launch plans' measure of a full device (132 on an H100 SXM when it cannot be read).
-int64_t num_sms() {
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-      sms <= 0)
-    sms = 132;
-  return sms;
 }
 
 }  // namespace

@@ -11,9 +11,9 @@
 // kernels are sized by the bound 3F and threads past E exit.  A face index outside [0, V) gives a key past every edge
 // and belongs to no edge.
 //
-// The adjacency.  The directed copies 2e + side of the E edges, keyed by their source vertex, sorted stably and offset
-// per vertex (run_offsets_kernel of mesh_tables.cuh), list each vertex's incident edges in edge order, which is also
-// ascending neighbour order; a self-loop (i, i) appears twice, as in the coalesced adjacency of laplacian().
+// The adjacency.  The directed copies 2e + side of the E edges, keyed by their source vertex and put into runs per
+// vertex (sort_into_runs of keyed_runs.cuh), list each vertex's incident edges in edge order, which is also ascending
+// neighbour order; a self-loop (i, i) appears twice, as in the coalesced adjacency of laplacian().
 //
 // cot and cotcurv walk the vertex -> corner table of mesh_tables.cuh: a corner's row of L is the cotangents of its
 // face's two other angles against the two other corners.
@@ -29,7 +29,6 @@
 namespace b200r {
 namespace {
 
-constexpr size_t kAlign = 256;
 constexpr int kReduceBlocksMax = 1024;
 constexpr float kCosEps = 1e-8f;       // torch.cosine_similarity's default eps
 constexpr float kAreaClamp = 1e-12f;   // cot_laplacian's eps
@@ -271,21 +270,13 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 
-// grad_verts[v] = the sum over v's incident edges, in edge order, of +rows[e] (v the edge's min) or -rows[e].
-__global__ void __launch_bounds__(kThreads)
-    edge_grad_verts_kernel(const int32_t* __restrict__ offsets, const int32_t* __restrict__ adjacency, int64_t V,
-                           const float* __restrict__ rows, float* __restrict__ grad_verts) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < V; v += stride) {
-    float3 acc = make_float3(0.0f, 0.0f, 0.0f);
-    for (int32_t i = offsets[v]; i < offsets[v + 1]; ++i) {
-      const int32_t d = adjacency[i];
-      const float3 r = load3(rows, d >> 1);
-      acc = (d & 1) ? sub3(acc, r) : add3(acc, r);
-    }
-    store3(grad_verts, v, acc);
-  }
-}
+// The row of directed copy d = 2e + side in the adjacency of v: rows[e], added where v is the edge's min (side 0) and
+// subtracted where it is the max.
+struct EdgeRows : AddedRows {
+  const float* rows;
+  __device__ float3 operator()(int64_t, int32_t d) const { return load3(rows, d >> 1); }
+  __device__ static bool negated(int32_t d) { return d & 1; }
+};
 
 // ---- Laplacian smoothing ------------------------------------------------------------------------------------------
 
@@ -631,52 +622,40 @@ struct Layout {
 
 bool layout(int64_t V, int64_t F, int N, Layout& L) {
   const size_t n3 = 3 * (size_t)F, n6 = 6 * (size_t)F, v = (size_t)V, nm = (size_t)(N > 0 ? N : 1);
-  size_t at = 0;
-  auto take = [&](size_t bytes) {
-    const size_t here = at;
-    at += align_up(bytes, kAlign);
-    return here;
-  };
-  L.tab = take(sizeof(int32_t) * (v + 1 + n6));
-  L.sorted = take(sizeof(int32_t) * n3);
-  L.run = take(sizeof(int32_t) * n3);
-  L.estart = take(sizeof(int32_t) * (n3 + 1));
-  L.edge_v = take(sizeof(int32_t) * 2 * n3);
-  L.nedges = take(sizeof(int32_t));
-  L.ebegin = take(sizeof(int32_t) * nm);
-  L.ecount = take(sizeof(int32_t) * nm);
-  L.pairs = take(sizeof(int64_t) * nm);
-  L.prefix = take(sizeof(int64_t) * (n3 + 1));
-  L.keys_in = take(sizeof(uint32_t) * n6);   // 3F 64-bit or 6F 32-bit keys
-  L.keys_out = take(sizeof(uint32_t) * n6);
-  L.ids_in = take(sizeof(int32_t) * n6);
-  L.fpos = take(sizeof(float) * 3 * n3);
-  L.ftmp = take(sizeof(float) * (3 * v > 3 * n3 ? 3 * v : 3 * n3));
-  L.fface = take(sizeof(float) * 9 * (size_t)F);
-  L.partials = take(sizeof(float) * kReduceBlocksMax);
-  L.cub = at;
+  Carver c;
+  L.tab = c.take(sizeof(int32_t) * (v + 1 + n6));
+  L.sorted = c.take(sizeof(int32_t) * n3);
+  L.run = c.take(sizeof(int32_t) * n3);
+  L.estart = c.take(sizeof(int32_t) * (n3 + 1));
+  L.edge_v = c.take(sizeof(int32_t) * 2 * n3);
+  L.nedges = c.take(sizeof(int32_t));
+  L.ebegin = c.take(sizeof(int32_t) * nm);
+  L.ecount = c.take(sizeof(int32_t) * nm);
+  L.pairs = c.take(sizeof(int64_t) * nm);
+  L.prefix = c.take(sizeof(int64_t) * (n3 + 1));
+  L.keys_in = c.take(sizeof(uint32_t) * n6);   // 3F 64-bit or 6F 32-bit keys
+  L.keys_out = c.take(sizeof(uint32_t) * n6);
+  L.ids_in = c.take(sizeof(int32_t) * n6);
+  L.fpos = c.take(sizeof(float) * 3 * n3);
+  L.ftmp = c.take(sizeof(float) * (3 * v > 3 * n3 ? 3 * v : 3 * n3));
+  L.fface = c.take(sizeof(float) * 9 * (size_t)F);
+  L.partials = c.take(sizeof(float) * kReduceBlocksMax);
   size_t need = 0, b = 0;
   const int bits = key_bits(V);
   if (n3 > 0) {
-    if (wide_keys(V)) {
-      if (cub::DeviceRadixSort::SortPairs(nullptr, b, (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                          (const int32_t*)nullptr, (int32_t*)nullptr, (int)n3, 0, 2 * bits) !=
-          cudaSuccess)
-        return false;
-    } else if (cub::DeviceRadixSort::SortPairs(nullptr, b, (const uint32_t*)nullptr, (uint32_t*)nullptr,
-                                               (const int32_t*)nullptr, (int32_t*)nullptr, (int)n3, 0, 2 * bits) !=
-               cudaSuccess) {
-      return false;
-    }
+    const bool sized = wide_keys(V) ? sort_bytes<uint64_t, int32_t>((int)n3, 2 * bits, b)
+                                    : sort_bytes<uint32_t, int32_t>((int)n3, 2 * bits, b);
+    if (!sized) return false;
     need = b > need ? b : need;
-    if (!corner_sort_bytes(V, n6, b)) return false;  // the adjacency; covers the corner table's 3F
+    if (!run_sort_bytes(V, (int64_t)n6, b)) return false;  // the adjacency; covers the corner table's 3F
     need = b > need ? b : need;
     if (cub::DeviceScan::InclusiveSum(nullptr, b, (const int64_t*)nullptr, (int64_t*)nullptr, (int)n3) != cudaSuccess)
       return false;
     need = b > need ? b : need;
   }
   L.cub_bytes = need;
-  L.total = L.cub + align_up(need, kAlign);
+  L.cub = c.take(need);
+  L.total = c.used;
   return true;
 }
 
@@ -694,14 +673,8 @@ int checked_layout(const char* op, int64_t V, int64_t F, int N, size_t workspace
                    Layout& L) {
   int rc = check_sizes(op, V, F, N);
   if (rc != B200R_OK) return rc;
-  if (!layout(V, F, N, L)) {
-    cudaGetLastError();
-    return fail(B200R_ERR_CUDA, std::string(op) + ": cub could not size its temporary storage");
-  }
-  if (workspace == nullptr || workspace_bytes < L.total)
-    return fail(B200R_ERR_INVALID_ARGUMENT,
-                std::string(op) + ": workspace smaller than b200r_regularizers_workspace_bytes");
-  return B200R_OK;
+  const bool sized = layout(V, F, N, L);
+  return check_workspace(op, "b200r_regularizers_workspace_bytes", sized, L.total, workspace, workspace_bytes);
 }
 
 struct Ws {
@@ -783,18 +756,13 @@ int build_edges(const int64_t* faces, int64_t V, int64_t F, const int64_t* first
 int build_adjacency(int64_t V, int64_t F, const Ws& w, cudaStream_t stream) {
   const int64_t n = 6 * F;
   uint32_t* keys_in = w.at<uint32_t>(w.L.keys_in);
-  uint32_t* keys_out = w.at<uint32_t>(w.L.keys_out);
   int32_t* ids_in = w.at<int32_t>(w.L.ids_in);
   if (n > 0) {
     adjacency_keys_kernel<<<grid_for(n), kThreads, 0, stream>>>(w.edge_v(), w.nedges(), n, V, keys_in, ids_in);
     B200R_LAUNCHED("adjacency_keys_kernel");
-    size_t cub_bytes = w.L.cub_bytes;
-    B200R_CUDA_OK(cub::DeviceRadixSort::SortPairs(w.cub(), cub_bytes, keys_in, keys_out, ids_in, w.tab() + V + 1,
-                                                  (int)n, 0, key_bits(V), stream));
   }
-  run_offsets_kernel<<<grid_for(n + 1), kThreads, 0, stream>>>(keys_out, n, V, w.tab());
-  B200R_LAUNCHED("run_offsets_kernel");
-  return B200R_OK;
+  return sort_into_runs(keys_in, w.at<uint32_t>(w.L.keys_out), ids_in, w.tab() + V + 1, n, V, w.cub(), w.L.cub_bytes,
+                        w.tab(), stream);
 }
 
 int build_corners(const int64_t* faces, int64_t V, int64_t F, const Ws& w, cudaStream_t stream) {
@@ -818,17 +786,14 @@ using namespace b200r;
 
 extern "C" size_t b200r_regularizers_workspace_bytes(int64_t V, int64_t F, int32_t N) {
   if (V < 0 || F < 0 || N < 0) return 0;
-  Layout L;
-  if (!layout(V, F, N, L)) {
-    cudaGetLastError();
-    return 0;
-  }
-  return L.total;
+  Layout L{};
+  const bool sized = layout(V, F, N, L);
+  return workspace_size(sized, L.total);
 }
 
 #define B200R_REG_PROLOGUE(op)                                                             \
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);                               \
-  Layout L;                                                                                \
+  Layout L{};                                                                              \
   int rc = checked_layout(op, V, F, N, workspace_bytes, workspace, L);                     \
   if (rc != B200R_OK) return rc;                                                           \
   const Ws w{static_cast<char*>(workspace), L};
@@ -888,8 +853,9 @@ extern "C" int b200r_mesh_edge_loss_backward(const float* grad_loss, const float
                                                                 target_length, w.fpos());
     B200R_LAUNCHED("edge_grad_rows_kernel");
   }
-  edge_grad_verts_kernel<<<grid_for(V), kThreads, 0, stream>>>(w.tab(), w.tab() + V + 1, V, w.fpos(), grad_verts);
-  B200R_LAUNCHED("edge_grad_verts_kernel");
+  segmented_sum_kernel<Mode::kSum>
+      <<<grid_for(V), kThreads, 0, stream>>>(w.tab(), w.tab() + V + 1, V, EdgeRows{{}, w.fpos()}, nullptr, grad_verts);
+  B200R_LAUNCHED("segmented_sum_kernel");
   return B200R_OK;
 }
 
@@ -1007,8 +973,9 @@ extern "C" int b200r_mesh_normal_consistency_backward(const float* grad_loss, co
     nc_corner_rows_kernel<<<grid_for(F), kThreads, 0, stream>>>(verts, faces, V, F, w.ftmp(), w.fface());
     B200R_LAUNCHED("nc_corner_rows_kernel");
   }
-  segmented_sum_kernel<RowOf::kCorner, Epilogue::kSum>
-      <<<grid_for(V), kThreads, 0, stream>>>(w.tab(), w.tab() + V + 1, V, F, w.fface(), nullptr, grad_verts);
+  segmented_sum_kernel<Mode::kSum>
+      <<<grid_for(V), kThreads, 0, stream>>>(w.tab(), w.tab() + V + 1, V, CornerRows<true>{{}, w.fface(), F}, nullptr,
+                                             grad_verts);
   B200R_LAUNCHED("segmented_sum_kernel");
   return B200R_OK;
 }

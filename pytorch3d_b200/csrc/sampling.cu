@@ -18,8 +18,8 @@
 // and a zero-area face has exactly the prefix of the face before it: it is never drawn.
 //
 // Backward: one thread per sample writes its three corner rows (w_j * grad_sample, plus the normalise and
-// cross-product backward of grad_normal) and keys them by vertex; a stable radix sort and the segmented sum of
-// mesh_tables.cuh add each vertex's rows in one thread, so there are no float atomics and the cost scales with the
+// cross-product backward of grad_normal) and keys them by vertex; sort_into_runs and the segmented sum of
+// keyed_runs.cuh add each vertex's rows in one thread, so there are no float atomics and the cost scales with the
 // samples, not the faces.
 #include "mesh_tables.cuh"
 
@@ -29,7 +29,6 @@ namespace {
 constexpr int kScanItems = 16;                                // faces per thread of the chunk scan
 constexpr int64_t kChunk = (int64_t)kThreads * kScanItems;   // 4096 faces per chunk
 constexpr int kWarps = kThreads / 32;
-constexpr size_t kAlign = 256;
 constexpr float kSampleNormalEps = 2.220446049250313e-16f;  // sys.float_info.epsilon, as clamp casts it to float32
 
 // Chunk slots of mesh m start at first[m] / kChunk + m: strictly increasing in m, and ceil(num[m] / kChunk) slots fit
@@ -273,26 +272,27 @@ struct Layout {
 
 bool layout(int64_t V, int64_t F, int64_t N, int64_t S, int pass, Layout& L) {
   L = Layout{};
+  Carver c;
   if (pass == 0) {
     const size_t slots = (size_t)num_slots(F, N);
-    L.prefix = 0;
-    L.chunk_total = L.prefix + align_up(sizeof(double) * (size_t)F, kAlign);
-    L.chunk_carry = L.chunk_total + align_up(sizeof(double) * slots, kAlign);
-    L.mesh_total = L.chunk_carry + align_up(sizeof(double) * slots, kAlign);
-    L.total = L.mesh_total + align_up(sizeof(double) * (size_t)N, kAlign);
+    L.prefix = c.take(sizeof(double) * (size_t)F);
+    L.chunk_total = c.take(sizeof(double) * slots);
+    L.chunk_carry = c.take(sizeof(double) * slots);
+    L.mesh_total = c.take(sizeof(double) * (size_t)N);
+    L.total = c.used;
     return true;
   }
   const size_t n = 3 * (size_t)N * (size_t)S;
-  L.rows = 0;
-  L.keys_in = L.rows + align_up(sizeof(float) * 3 * n, kAlign);
-  L.keys_out = L.keys_in + align_up(sizeof(uint32_t) * n, kAlign);
-  L.ids_in = L.keys_out + align_up(sizeof(uint32_t) * n, kAlign);
-  L.corners = L.ids_in + align_up(sizeof(int32_t) * n, kAlign);
-  L.offsets = L.corners + align_up(sizeof(int32_t) * n, kAlign);
-  L.cub = L.offsets + align_up(sizeof(int32_t) * ((size_t)V + 1), kAlign);
-  if (!corner_sort_bytes(V, n, L.cub_bytes)) return false;
-  L.total = L.cub + align_up(L.cub_bytes, kAlign);
-  return true;
+  L.rows = c.take(sizeof(float) * 3 * n);
+  L.keys_in = c.take(sizeof(uint32_t) * n);
+  L.keys_out = c.take(sizeof(uint32_t) * n);
+  L.ids_in = c.take(sizeof(int32_t) * n);
+  L.corners = c.take(sizeof(int32_t) * n);
+  L.offsets = c.take(sizeof(int32_t) * ((size_t)V + 1));
+  const bool sized = run_sort_bytes(V, (int64_t)n, L.cub_bytes);
+  L.cub = c.take(L.cub_bytes);
+  L.total = c.used;
+  return sized;
 }
 
 int check_sizes(const char* op, int64_t V, int64_t F, int64_t N, int64_t S, bool backward) {
@@ -307,14 +307,8 @@ int check_sizes(const char* op, int64_t V, int64_t F, int64_t N, int64_t S, bool
 
 int checked_layout(const char* op, int64_t V, int64_t F, int64_t N, int64_t S, int pass, size_t workspace_bytes,
                    const void* workspace, Layout& L) {
-  if (!layout(V, F, N, S, pass, L)) {
-    cudaGetLastError();
-    return fail(B200R_ERR_CUDA, std::string(op) + ": cub could not size the sort's temporary storage");
-  }
-  if (workspace == nullptr || workspace_bytes < L.total)
-    return fail(B200R_ERR_INVALID_ARGUMENT,
-                std::string(op) + ": workspace smaller than b200r_sample_points_workspace_bytes");
-  return B200R_OK;
+  const bool sized = layout(V, F, N, S, pass, L);
+  return check_workspace(op, "b200r_sample_points_workspace_bytes", sized, L.total, workspace, workspace_bytes);
 }
 
 }  // namespace
@@ -325,11 +319,8 @@ using namespace b200r;
 extern "C" size_t b200r_sample_points_workspace_bytes(int64_t V, int64_t F, int64_t N, int64_t S, int32_t pass) {
   if (V < 0 || F < 0 || N < 1 || S < 1 || (pass != 0 && pass != 1)) return 0;
   Layout L;
-  if (!layout(V, F, N, S, pass, L)) {
-    cudaGetLastError();
-    return 0;
-  }
-  return L.total;
+  const bool sized = layout(V, F, N, S, pass, L);
+  return workspace_size(sized, L.total);
 }
 
 extern "C" int b200r_sample_points_forward(const float* verts, int64_t V, const int64_t* faces, int64_t F,
@@ -402,13 +393,11 @@ extern "C" int b200r_sample_points_backward(const float* grad_samples, const flo
     corner_rows_kernel<false><<<grid_for(M), kThreads, 0, stream>>>(grad_samples, nullptr, verts, V, faces, F,
                                                                     face_idx, bary, M, rows, keys_in, ids_in);
   B200R_LAUNCHED("corner_rows_kernel");
-  B200R_CUDA_OK(cub::DeviceRadixSort::SortPairs(ws + L.cub, L.cub_bytes, keys_in, keys_out, ids_in, corners, (int)n, 0,
-                                                key_bits(V), stream));
-  run_offsets_kernel<<<grid_for(n + 1), kThreads, 0, stream>>>(keys_out, n, V, offsets);
-  B200R_LAUNCHED("run_offsets_kernel");
-  // corner id c = j * M + g: segmented_sum_kernel's (j, f) decoding with F = M, rows (g, j)
-  segmented_sum_kernel<RowOf::kCorner, Epilogue::kSum>
-      <<<grid_for(V), kThreads, 0, stream>>>(offsets, corners, V, M, rows, nullptr, grad_verts);
+  rc = sort_into_runs(keys_in, keys_out, ids_in, corners, n, V, ws + L.cub, L.cub_bytes, offsets, stream);
+  if (rc != B200R_OK) return rc;
+  // corner id c = j * M + g, rows (g, j)
+  segmented_sum_kernel<Mode::kSum>
+      <<<grid_for(V), kThreads, 0, stream>>>(offsets, corners, V, CornerRows<true>{{}, rows, M}, nullptr, grad_verts);
   B200R_LAUNCHED("segmented_sum_kernel");
   return B200R_OK;
 }

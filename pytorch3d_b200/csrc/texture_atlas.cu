@@ -16,14 +16,11 @@
 // are no float atomics: a key pass gives each slot the index of the cell it sampled (or a sentinel when its
 // contribution is exactly ±0 in every channel, or the cell is out of range), a stable radix sort orders the
 // (cell, slot) pairs, and a segmented pass sums each cell's run in ascending slot order from +0 and writes it once.
-#include <cub/device/device_radix_sort.cuh>
-
-#include "common.cuh"
+#include "keyed_runs.cuh"
 
 namespace b200r {
 namespace {
 
-constexpr int kThreads = 256;
 constexpr uint32_t kBackgroundBit = 0x80000000u;  // in the sorted slot index: the slot's texel was multiplied by 0
 
 struct AtlasGeometry {
@@ -133,58 +130,44 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 
-// ceil(log2(cells + 1)): the key bits the sort looks at (the sentinel, `cells`, included).
-int key_bits(int64_t cells) {
-  int bits = 1;
-  while (bits < 64 && (cells >> bits) != 0) ++bits;
-  return bits;
-}
+// Workspace layout: keys in / out, slot indices in / out, then cub's temporary storage of a sort over key_bits(cells)
+// bits.  Returns false when cub cannot size its storage (no device).
+struct Layout {
+  size_t keys_in, keys_out, slots_in, slots_out, cub, cub_bytes, total;
+};
 
-constexpr size_t kAlign = 256;
-
-// Workspace layout: keys in / out, slot indices in / out, then cub's temporary storage.  Returns false when cub cannot
-// size its storage (no device).
 template <typename KeyT>
-bool workspace_layout(int64_t total, int bits, size_t& cub_offset, size_t& cub_bytes, size_t& total_bytes,
-                      size_t offsets[4]) {
-  const size_t kb = align_up(sizeof(KeyT) * (size_t)total, kAlign), vb = align_up(sizeof(uint32_t) * (size_t)total,
-                                                                                    kAlign);
-  offsets[0] = 0;
-  offsets[1] = kb;
-  offsets[2] = 2 * kb;
-  offsets[3] = 2 * kb + vb;
-  cub_offset = 2 * kb + 2 * vb;
-  cub_bytes = 0;
-  if (cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const KeyT*)nullptr, (KeyT*)nullptr,
-                                      (const uint32_t*)nullptr, (uint32_t*)nullptr, total, 0, bits) != cudaSuccess)
-    return false;
-  total_bytes = cub_offset + align_up(cub_bytes, kAlign);
-  return true;
+bool layout(int64_t total, int64_t cells, Layout& L) {
+  Carver c;
+  L.keys_in = c.take(sizeof(KeyT) * (size_t)total);
+  L.keys_out = c.take(sizeof(KeyT) * (size_t)total);
+  L.slots_in = c.take(sizeof(uint32_t) * (size_t)total);
+  L.slots_out = c.take(sizeof(uint32_t) * (size_t)total);
+  const bool sized = sort_bytes<KeyT, uint32_t>(total, key_bits(cells), L.cub_bytes);
+  L.cub = c.take(L.cub_bytes);
+  L.total = c.used;
+  return sized;
 }
 
 template <typename KeyT>
 int backward_sorted(const AtlasGeometry& g, const float* grad_texels, int64_t cells, void* workspace,
                     size_t workspace_bytes, float* grad_atlas, cudaStream_t stream) {
-  const int bits = key_bits(cells);
-  size_t cub_offset, cub_bytes, need, off[4];
-  if (!workspace_layout<KeyT>(g.total, bits, cub_offset, cub_bytes, need, off)) {
-    cudaGetLastError();
-    return fail(B200R_ERR_CUDA, "texture_atlas_backward: cub could not size the sort's temporary storage");
-  }
-  if (workspace == nullptr || workspace_bytes < need)
-    return fail(B200R_ERR_INVALID_ARGUMENT, "texture_atlas_backward: workspace smaller than "
-                                            "b200r_texture_atlas_workspace_bytes");
+  Layout L;
+  const bool sized = layout<KeyT>(g.total, cells, L);
+  const int rc = check_workspace("texture_atlas_backward", "b200r_texture_atlas_workspace_bytes", sized, L.total,
+                                 workspace, workspace_bytes);
+  if (rc != B200R_OK) return rc;
   char* ws = static_cast<char*>(workspace);
-  KeyT* keys_in = reinterpret_cast<KeyT*>(ws + off[0]);
-  KeyT* keys_out = reinterpret_cast<KeyT*>(ws + off[1]);
-  uint32_t* slots_in = reinterpret_cast<uint32_t*>(ws + off[2]);
-  uint32_t* slots_out = reinterpret_cast<uint32_t*>(ws + off[3]);
+  KeyT* keys_in = reinterpret_cast<KeyT*>(ws + L.keys_in);
+  KeyT* keys_out = reinterpret_cast<KeyT*>(ws + L.keys_out);
+  uint32_t* slots_in = reinterpret_cast<uint32_t*>(ws + L.slots_in);
+  uint32_t* slots_out = reinterpret_cast<uint32_t*>(ws + L.slots_out);
   const KeyT sentinel = (KeyT)cells;
-  const dim3 grid((unsigned)cap_grid_stride_blocks((g.total + kThreads - 1) / kThreads));
+  const dim3 grid = grid_for(g.total);
   texture_atlas_keys_kernel<KeyT><<<grid, kThreads, 0, stream>>>(g, grad_texels, sentinel, keys_in, slots_in);
   B200R_LAUNCHED("texture_atlas_keys_kernel");
-  B200R_CUDA_OK(cub::DeviceRadixSort::SortPairs(ws + cub_offset, cub_bytes, keys_in, keys_out, slots_in, slots_out,
-                                                g.total, 0, bits, stream));
+  B200R_CUDA_OK(cub::DeviceRadixSort::SortPairs(ws + L.cub, L.cub_bytes, keys_in, keys_out, slots_in, slots_out,
+                                                g.total, 0, key_bits(cells), stream));
 #define B200R_ATLAS_LAUNCH(CT)                                                                                     \
   texture_atlas_reduce_kernel<KeyT, CT><<<grid, kThreads, 0, stream>>>(keys_out, slots_out, g.total, sentinel, g.C, \
                                                                        grad_texels, grad_atlas);
@@ -214,15 +197,9 @@ extern "C" size_t b200r_texture_atlas_workspace_bytes(int32_t N, int32_t H, int3
                                                       int32_t R) {
   const int64_t total = (int64_t)N * H * W * K, cells = F * R * (int64_t)R;
   if (total <= 0 || cells <= 0 || R < 1) return 0;
-  size_t cub_offset, cub_bytes, need = 0, off[4];
-  const int bits = key_bits(cells);
-  const bool ok = bits > 32 ? workspace_layout<uint64_t>(total, bits, cub_offset, cub_bytes, need, off)
-                            : workspace_layout<uint32_t>(total, bits, cub_offset, cub_bytes, need, off);
-  if (!ok) {
-    cudaGetLastError();
-    return 0;
-  }
-  return need;
+  Layout L;
+  const bool sized = key_bits(cells) > 32 ? layout<uint64_t>(total, cells, L) : layout<uint32_t>(total, cells, L);
+  return workspace_size(sized, L.total);
 }
 
 extern "C" int b200r_texture_atlas_forward(const int64_t* pix_to_face, const float* barycentric_coords,
@@ -234,7 +211,7 @@ extern "C" int b200r_texture_atlas_forward(const int64_t* pix_to_face, const flo
   const int64_t total = (int64_t)N * H * W * K;
   if (total == 0) return B200R_OK;
   const AtlasGeometry g{pix_to_face, barycentric_coords, total, F, R, C};
-  const dim3 grid((unsigned)cap_grid_stride_blocks((total + kThreads - 1) / kThreads));
+  const dim3 grid = grid_for(total);
   switch (C) {
     case 1: texture_atlas_forward_kernel<1><<<grid, kThreads, 0, stream>>>(g, atlas, texels); break;
     case 2: texture_atlas_forward_kernel<2><<<grid, kThreads, 0, stream>>>(g, atlas, texels); break;
